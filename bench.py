@@ -5,7 +5,7 @@
     torchrun --nproc-per-node N bench.py --gpus N ...           (one rank per GPU)
     python bench.py --impl reference ...                         (the reference's CPU path, see below)
 
-One "step" = one pass of the hot path over one batch per GPU: yb_forward (tcgen05 fp16 network + DFL/box
+One "step" = one pass of the hot path over one batch per GPU: yb_forward (wgmma fp16 network + DFL/box
 decode) -> yb_nms (GPU NMS) [-> all-gather of the fixed-capacity detection payloads when N > 1: by default the
 library's own peer-memory exchange (yb_comm_*, NVLink stores + flags, no NCCL kernel on the path), `--gather nccl`
 for one packed ncclAllGather].  Workload at N=1 = BASELINE.json configs[1]: YOLOv8n detect, batch 32 x 3x640x640.
@@ -17,7 +17,7 @@ Printed JSON (one line, rank 0):
              test images (v8n only; tests/golden fixtures)
   e2e        same metric through the host-buffer C-ABI calls yb_predict_u8_submit/_wait (pinned uint8 images in,
              detections out; H2D + D2H - and at N > 1 the detection gather - inside the timed region)
-  roofline   the dominant kernel (conv_tc_kernel, the tcgen05 implicit-GEMM conv): algorithmic FLOPs and bytes of all
+  roofline   the dominant kernel (conv_tc_kernel, the wgmma implicit-GEMM conv): algorithmic FLOPs and bytes of all
              its launches in one step / the time they take INSIDE the graph-replayed forward = event-timed forward
              minus the other kernels of the forward (stem / pool / upsample, each timed back to back with yb_time_op).
              kernel_ms_per_step <= forward_ms_per_step <= ms_per_step by construction.
@@ -54,7 +54,7 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tc_burst=d["bf16_tflops"], tc=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tc_burst=1590.0, tc=1400.0, src="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, tc_burst=989.0, tc=989.0, src="H100 SXM data sheet (dense fp16 / bf16), not measured")
 
 
 class ClockSampler:
@@ -102,6 +102,38 @@ class ClockSampler:
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "samples": len(sm), "reasons": sorted(reasons)}
+
+
+DUMP_CAP = 64 << 20  # bytes of .npy payload --dump-outputs may write
+
+
+def dump_outputs(out_dir, arrays):
+    """Write the arrays a caller of the timed path receives from its last step as DIR/<name>.npy (float32 / float64).
+    Arrays that would not fit DUMP_CAP are sampled by the caller; the total is checked here."""
+    import numpy as np
+    total = sum(a.numel() * a.element_size() for a in arrays.values())
+    assert total <= DUMP_CAP, f"--dump-outputs: {total} bytes exceed {DUMP_CAP}"
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
+
+
+def infer_dump_arrays(last):
+    """Inference: detections, counts and NMS indices as returned; the prediction tensor (B, 4 + nc [+ 32], 8400 anchors,
+    86 MB at batch 32) as a fixed seeded sample of anchors, as many as fit DUMP_CAP beside the rest (at most 2048);
+    instance masks (segment): the first 16 detections of every image, every 16th pixel."""
+    import torch
+    arrays = {"detections": last["detections"].float(), "counts": last["counts"].double(), "keep": last["keep"].double()}
+    if "masks" in last:
+        arrays["masks_sample"] = last["masks"][:, :16, ::16, ::16].float()
+    pred = last["pred"]
+    B, Cp, A = pred.shape
+    rest = sum(a.numel() * a.element_size() for a in arrays.values())
+    n = min(2048, A, (DUMP_CAP - rest) // (B * Cp * 4 + 8))
+    idx = torch.randperm(A, generator=torch.Generator().manual_seed(0))[:n].sort().values
+    arrays["pred_sample"] = pred[..., idx.to(pred.device)].float()
+    arrays["pred_sample_anchors"] = idx.double()
+    return arrays
 
 
 def cpu_reference_run(model_key, batch, steps, warmup):
@@ -212,7 +244,7 @@ def synth_targets(B, seed):
 def train_main(args, rank, world, local_rank):
     """BASELINE configs[3]: YOLOv11s training step (train-mode forward with batch-statistics BatchNorm, v8DetectionLoss
     incl. the task-aligned assigner, backward through the whole graph, ONE NCCL all-reduce of the flat gradient buffer
-    when N > 1, AdamW), batch 16 per GPU.  Dense convolutions (forward, dgrad, wgrad) run on the TF32 tcgen05 kernels
+    when N > 1, AdamW), batch 16 per GPU.  Dense convolutions (forward, dgrad, wgrad) run on the TF32 tensor-core kernels
     (csrc/conv_tf32.cu; --train-kernels f32 times the fp32 CUDA-core parity kernels instead); depthwise convolutions,
     attention, BatchNorm / SiLU, the loss and AdamW are fp32 CUDA-core kernels of the library."""
     model = args.model if args.model.startswith("v11") else "v11s"
@@ -260,7 +292,7 @@ def train_main(args, rank, world, local_rank):
     import torch.distributed as dist
     from tests.util import oracle_model, synth_image
     from yolosharp_b200.train_v11 import KernelOpsV11, TrainStepV11
-    assert torch.cuda.is_available(), "bench.py needs a B200"
+    assert torch.cuda.is_available(), "bench.py needs an H100"
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -295,6 +327,8 @@ def train_main(args, rank, world, local_rank):
             print(f"step {i}: {(time.perf_counter() - _t0) * 1e3:.1f} ms", file=sys.stderr)
     e1.record()
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:  # what the step returns to its caller: the loss items of the last timed step
+        dump_outputs(args.dump_outputs, {"loss_items": items.detach().double()})
     if world > 1:
         dist.barrier()
     t = torch.tensor([e0.elapsed_time(e1)], device=dev)
@@ -356,7 +390,7 @@ def train_main(args, rank, world, local_rank):
                           "loss_items": [round(float(v), 4) for v in host_items],
                           "roofline": {"bound": "tensor", "achieved": round(tflops, 2), "peak": peaks["tc"], "unit": "TFLOP/s",
                                        "frac": round(tflops / peaks["tc"], 5), "traffic": None,
-                                       "kernel": "tf_conv_kernel / tf_wgrad_kernel (TF32 tcgen05)" if tc else
+                                       "kernel": "tf_conv_kernel / tf_wgrad_kernel (TF32 tensor cores)" if tc else
                                                  "conv_generic / conv_backward_data / conv_backward_weight (fp32 CUDA cores)",
                                        "note": "whole-step figure: 3 x forward conv FLOPs / step time, against the sustained "
                                                "bf16 tensor peak (TF32 peaks at half of it); the step also holds the fp32 "
@@ -378,11 +412,15 @@ def main():
     ap.add_argument("--train-impl", default="native", choices=["native", "python"],
                     help="--mode train: the native step (csrc/train_step.cu) or the Python graph walk over the same kernels")
     ap.add_argument("--train-kernels", default="tc", choices=["tc", "f32"],
-                    help="--mode train: dense convolutions on the TF32 tcgen05 kernels (default) or the fp32 parity kernels")
+                    help="--mode train: dense convolutions on the TF32 tensor-core kernels (default) or the fp32 parity kernels")
     ap.add_argument("--mode", default="infer", choices=["infer", "train"],
                     help="train: one YOLOv11s training step (fwd + v8DetectionLoss + bwd + all-reduce + AdamW), BASELINE configs[3]")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-real-weights", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned to its caller to DIR/<name>.npy, float32 / float64, "
+                         "<= 64 MB: inference - detections, NMS indices, a seeded sample of the prediction tensor and of "
+                         "the masks; --mode train - the loss items")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))
@@ -418,7 +456,7 @@ def main():
     import yolosharp_b200 as y
     from yolosharp_b200 import dist as ydist
     from tests.util import oracle_model, synth_image
-    assert torch.cuda.is_available(), "bench.py needs a B200 (no CPU fallback in the product path)"
+    assert torch.cuda.is_available(), "bench.py needs an H100 (no CPU fallback in the product path)"
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     torch.cuda.init()
@@ -442,10 +480,11 @@ def main():
     A, Cp = eng.anchors, eng.pred_channels
     gatherer = ydist.DetectionGather(B, MAX_DET, ROW, dev, mode=args.gather, slots=max(2, E2E_SLOTS)) if world > 1 else None
 
-    def timed_run(eng, xs, steps, warmup, with_gather):
+    def timed_run(eng, xs, steps, warmup, with_gather, keep_last=False):
         """Two-deep software pipeline: forward(i+1) runs on stream s_f while NMS (+ masks, + gather) of batch i runs on
         stream s_n, each with its own prediction / detection buffers - every step does all of its work inside the
-        timed region.  Returns (ms_total over `steps`, mean detections per image, last pred buffer)."""
+        timed region.  Returns (ms_total over `steps`, mean detections per image, last pred buffer, forward ms per step,
+        with keep_last, a copy of what the last timed step returned to its caller, else None)."""
         s_f, s_n = torch.cuda.Stream(dev, priority=-1), torch.cuda.Stream(dev, priority=-1)
         preds = [torch.empty((B, Cp, A), dtype=torch.float32, device=dev) for _ in range(2)]
         protos = [torch.empty((B, 32, 160, 160), dtype=torch.float32, device=dev) for _ in range(2)] if seg else None
@@ -484,6 +523,14 @@ def main():
         s_f.wait_stream(s_n)
         e1.record(s_f)
         torch.cuda.synchronize()
+        last = None
+        if keep_last:
+            b = (steps - 1) & 1
+            # at N > 1 a caller receives the detections of every rank (the gathered window), NMS indices stay local
+            dets, counts = gatherer.gathered(b) if with_gather else detb[b][:2]
+            last = {"pred": preds[b].clone(), "detections": dets.clone(), "counts": counts.clone(), "keep": keepb[b].clone()}
+            if seg:
+                last["masks"] = mask_buf[b].clone()
         if world > 1:
             dist.barrier()
         t = torch.tensor([e0.elapsed_time(e1)], device=dev)
@@ -496,14 +543,18 @@ def main():
             eng.forward(xs[i % len(xs)], preds[i & 1], protos[i & 1] if seg else None, stream=s_f)
         f1.record(s_f)
         torch.cuda.synchronize()
-        return float(t.item()), float(detb[0][1].float().mean().item()), preds[0], f0.elapsed_time(f1) / steps
+        return float(t.item()), float(detb[0][1].float().mean().item()), preds[0], f0.elapsed_time(f1) / steps, last
 
     xs = [synth_image(B, 640, 640, seed=100 + rank * 8 + i, dtype=torch.float16).to(dev) for i in range(4)]
     sampler = ClockSampler(local_rank) if rank == 0 else None
     if sampler:
         sampler.start()
-    ms_total, mean_dets, pred, fwd_ms = timed_run(eng, xs, args.steps, args.warmup, world > 1)
+    ms_total, mean_dets, pred, fwd_ms, last = timed_run(eng, xs, args.steps, args.warmup, world > 1,
+                                                         keep_last=bool(args.dump_outputs) and rank == 0)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, infer_dump_arrays(last))
+    del last
     value = world * B * args.steps / (ms_total / 1e3)
 
     # ---- the same measurement on the reference's shipped checkpoint + its test images (v8n detect only) ----
@@ -516,7 +567,7 @@ def main():
             eng_r = make_engine({k: torch.from_numpy(z[k]) for k in z.files})
             u8 = image_batch(B)
             xr = [torch.roll(u8, shifts=i, dims=0).to(dev) for i in range(4)]  # uint8 input: /255 fused into the stem
-            ms_r, dets_r, _, fwd_r = timed_run(eng_r, xr, max(10, args.steps // 2), args.warmup, False)
+            ms_r, dets_r, _, fwd_r, _ = timed_run(eng_r, xr, max(10, args.steps // 2), args.warmup, False)
             real = {"value": round(B * max(10, args.steps // 2) / (ms_r / 1e3), 1), "unit": "images/s",
                     "weights": "reference Yolov8n.bin (tests/golden/yolov8n_f16.npz)",
                     "inputs": "32 x 640x640 uint8 built from the reference's 5 test images (pad 114, rolled copies)",
@@ -531,7 +582,7 @@ def main():
     e2e_val, e2e_steps, d2h = None, 0, 0
     if not (seg and world > 1):
         NS = E2E_SLOTS
-        torch.set_num_threads(1)  # the serving loop is ctypes calls only; idle intra-op workers cost it 15 % (profiles/r2_exp_e2e_matrix.txt)
+        torch.set_num_threads(1)  # the serving loop is ctypes calls only; idle intra-op workers would compete with it
         host["omp_threads_e2e"] = 1
         u8 = [synth_image(B, 640, 640, seed=200 + rank * 8 + i, dtype=torch.uint8).pin_memory() for i in range(NS)]
         GB = world * B if world > 1 else B
@@ -601,12 +652,7 @@ def main():
     tc_flops = sum(r["flops"] for r in tc)
     tc_bytes = sum(r["bytes"] for r in tc)
     tc_ms = max(fwd_ms - other_ms, 1e-6)
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r2_conv_traffic.json")
-    if os.path.exists(tpath):  # dram bytes of the same launches from an ncu capture (tools/ncu_traffic.py)
-        tj = json.load(open(tpath))
-        if tj.get("model") == args.model and tj.get("batch") == B:
-            traffic = tj["dram_bytes_per_step"]
+    traffic = None  # DRAM bytes of the conv launches need a profiler capture (tools/ncu_traffic.py); the bench takes none
     t_tc = tc_flops / (peaks["tc"] * 1e12)
     t_hbm = tc_bytes / (peaks["hbm"] * 1e9)
     if t_hbm >= t_tc:

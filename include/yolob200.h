@@ -1,5 +1,5 @@
 /*
- * yolob200.h - C ABI of the B200-native YOLO forward / NMS engine.
+ * yolob200.h - C ABI of the H100-native YOLO forward / NMS engine.
  *
  * This is the drop-in boundary for the hot path of IntptrMax/YoloSharp (reference
  * @16dc3cd, paths below relative to /root/reference/YoloSharp).  The reference has no
@@ -45,7 +45,7 @@ typedef enum { YB_TASK_DETECT = 0, YB_TASK_SEGMENT = 1 } yb_task;
 /* arithmetic mode of the network body */
 typedef enum {
   YB_PREC_F32 = 0, /* parity mode: fp32 storage + fp32 FMA (matches the fp32 oracle to ~1e-5) */
-  YB_PREC_F16 = 1  /* throughput mode: fp16 NHWC storage, tcgen05 tensor-core MMA, fp32 accumulate */
+  YB_PREC_F16 = 1  /* throughput mode: fp16 NHWC storage, wgmma tensor-core MMA, fp32 accumulate */
 } yb_precision;
 
 /* element types of caller buffers; values are torch ScalarType codes as stored in the
@@ -66,7 +66,7 @@ typedef struct {
   int32_t flags;      /* YB_FLAG_* */
 } yb_config;
 
-#define YB_FLAG_NO_TCGEN05 1  /* F16 mode: use the CUDA-core fp16 kernels instead of tcgen05 (debug) */
+#define YB_FLAG_NO_TCGEN05 1  /* F16 mode: use the CUDA-core fp16 kernels instead of the tensor-core kernels (debug) */
 #define YB_FLAG_NO_GRAPH   2  /* do not capture the forward into a CUDA graph */
 #define YB_FLAG_NO_CONCURRENCY 8  /* run the independent head branches serially on one stream */
 #define YB_FLAG_DRY_RUN    4  /* build the op graph / expected-tensor list only (no CUDA calls; for host-side checks).
@@ -216,7 +216,7 @@ int32_t yb_conv_backward_weight(const float* x, const float* dz, int32_t n, int3
 
 /* Replaces (training path, tensor cores): the same three convolution passes as the fp32 parity kernels above -
  * `Conv2d.forward` and the dgrad / wgrad libtorch runs behind `loss.backward()` (Modules/Convs.cs:44,
- * Utils/Amp.cs:260-286) - as tcgen05 implicit GEMMs with TF32 operands and fp32 accumulation (the arithmetic class of
+ * Utils/Amp.cs:260-286) - as tensor-core implicit GEMMs with TF32 operands and fp32 accumulation (the arithmetic class of
  * libtorch's own CUDA convolutions, whose cuDNN path allows TF32 by default).  Same tensors and layouts as
  * yb_conv_forward_f32 / yb_conv_backward_*, except that `w` is always the checkpoint layout (Cout, Cin, k, k).
  * Supported: cin % 8 == 0, cout % 8 == 0, k in {1, 3}, stride in {1, 2}, pad == k / 2 (stride-2 dgrad: even height /
@@ -247,7 +247,7 @@ int32_t yb_stem_conv_backward_weight_f32(const float* x, int32_t x_channels, con
 
 /* Replaces: `AMPWrapper.TrainStep` (Utils/Amp.cs:260-286: yolo.forward -> loss -> loss.backward() -> optimizer.step()) for
  * the YOLOv8 / YOLOv11 detect models as ONE call (csrc/train_step.cu): train-mode forward with batch-statistics
- * BatchNorm, v8DetectionLoss, backward through the whole graph (TF32 tcgen05 convolutions), AdamW per name group
+ * BatchNorm, v8DetectionLoss, backward through the whole graph (TF32 tensor-core convolutions), AdamW per name group
  * (YoloBaseTaskModel.cs:142-160: the "bias" group first).
  *   yb_trainer_create   cfg: arch (8 | 11), size, nc, device, max_batch, height, width (task detect);
  *                       flags & YB_FLAG_DRY_RUN builds the parameter layout only (no device memory)
@@ -471,9 +471,9 @@ int32_t yb_time_op(yb_engine* e, int32_t op_index, const void* in, int32_t in_dt
 /* Algorithmic work of op i for `batch` images: flops = 2*MACs (convs only), bytes = input view +
  * output view (+ residual) + weights, each counted once (SURVEY.md section 8(d) definitions). */
 int32_t yb_op_cost(const yb_engine* e, int32_t op_index, int32_t batch, double* flops, double* bytes);
-/* 0 = tcgen05 conv, 1 = CUDA-core conv, 2 = stem, 3 = depthwise, 4 = pool, 5 = upsample, 6 = decode, 7 = other */
+/* 0 = tensor-core conv, 1 = CUDA-core conv, 2 = stem, 3 = depthwise, 4 = pool, 5 = upsample, 6 = decode, 7 = other */
 int32_t yb_op_kind(const yb_engine* e, int32_t op_index);
-/* debug: the `skip`-th tcgen05 conv launch from now records a clock64 timeline of CTA 0 into dev_buf (128 x int64) */
+/* debug: the `skip`-th tensor-core conv launch from now records a clock64 timeline of CTA 0 into dev_buf (128 x int64) */
 int32_t yb_debug_timeline(long long* dev_buf, int32_t skip);
 
 #ifdef __cplusplus

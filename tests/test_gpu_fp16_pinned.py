@@ -1,4 +1,4 @@
-"""GPU parity of the BENCHED mode (fp16 storage + tcgen05, YB_PREC_F16) against the fp16-emulating oracle
+"""GPU parity of the BENCHED mode (fp16 storage + tensor cores, YB_PREC_F16) against the fp16-emulating oracle
 (oracle/emul16.py), at the benched shape and on the reference's shipped checkpoint.
 
 Two gaps are stated separately:
@@ -24,9 +24,8 @@ from tests.util import (GOLDEN, expected_for_op, oracle_activations, oracle_mode
 pytestmark = pytest.mark.gpu
 
 # Per stored layer, engine vs emulating oracle.  One fp16 ulp at the top of a layer's range is 2^-10 = 9.8e-4 of that
-# range, so ANY one-ulp flip of a large element already costs ~1e-3 on the max metric; observed on B200: 2.4e-4 (stem)
-# growing to 2.5e-3 in the deepest head layers as flips propagate, identical with the exact two-MUFU SiLU
-# (profiles/r2_parity_fp16_emul.txt) - it is the fp16 storage noise floor, not an arithmetic difference.
+# range, so ANY one-ulp flip of a large element already costs ~1e-3 on the max metric; the error grows from the stem to
+# the deepest head layers as flips propagate - it is the fp16 storage noise floor, not an arithmetic difference.
 EMUL_LAYER_TOL = 3e-3   # max |diff| / layer range  (3 fp16 ulps at the top of the range)
 EMUL_LAYER_RMS = 3e-4   # rms diff / layer range
 # Prediction tensor: the final 1x1 convs (64 / 80 inputs) and the DFL expectation (x stride) amplify that noise on
@@ -101,7 +100,7 @@ def assert_pred_close(pred, ref, box_tol, cls_tol, scale=1.0):
 
 
 def test_fp16_layers_vs_emulating_oracle_real_weights_640(y):
-    """Shipped Yolov8n checkpoint, 4 real 640x640 images, uint8 input path: every stored layer of the tcgen05
+    """Shipped Yolov8n checkpoint, 4 real 640x640 images, uint8 input path: every stored layer of the tensor-core
     engine within EMUL_LAYER_TOL of the emulating oracle; the fp16 -> fp32 gap is reported separately."""
     m, sd = oracle_real_v8n()
     m16 = emul16.convert(m)
@@ -123,7 +122,7 @@ def test_fp16_layers_vs_emulating_oracle_real_weights_640(y):
 
 
 def test_fp16_benched_shape_32x640_real_weights(y):
-    """BASELINE configs[1] shape (32x3x640x640, fp16 tcgen05) on the shipped checkpoint: prediction tensor within
+    """BASELINE configs[1] shape (32x3x640x640, fp16 tensor-core) on the shipped checkpoint: prediction tensor within
     tolerance of the emulating oracle, NMS (conf 0.25 / iou 0.45) keeps the same anchors with the same classes."""
     m, sd = oracle_real_v8n()
     m16 = emul16.convert(m)
@@ -183,7 +182,7 @@ def test_fp16_detector_all_test_images_vs_golden(y):
 @pytest.mark.parametrize("size,task", [("x", "detect"), ("s", "segment")])
 def test_wide_models_640_both_modes(y, size, task):
     """v8x (configs[2]) and v8s-seg (configs[4]) at 640x640: fp32 parity mode within 1e-3 of the fp32 oracle,
-    fp16 tcgen05 mode within the emulating-oracle tolerance."""
+    fp16 tensor-core mode within the emulating-oracle tolerance."""
     m = oracle_model("v8", task, size)
     x = synth_image(1, 640, 640)
     with torch.no_grad():

@@ -1,10 +1,10 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path, called through the C ABI, against
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C ABI, against
 the oracle on the same seeded inputs.
 
 Tolerances (BASELINE.json north_star: 1e-3 fp32, indices bit-exact):
   * NMS (integer/index work + fp32 arithmetic restated op by op): bit-exact rows and indices.
   * fp32 parity mode: prediction tensor within rtol/atol 1e-3 of the fp32 oracle (observed ~1e-5).
-  * fp16 tcgen05 mode: fp16 storage + fp16 MMA operands perturb activations at the 1e-3..1e-2
+  * fp16 tensor-core mode: fp16 storage + fp16 MMA operands perturb activations at the 1e-3..1e-2
     level, so it is checked per layer at 3e-2 of the layer's range and on the detections with set
     matching - it cannot meet 1e-3 and neither does the reference's own fp16 path (SURVEY.md §7).
 """
@@ -24,7 +24,7 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope="module")
 def y():
     import yolosharp_b200
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     from yolosharp_b200 import _lib
     _lib.lib()
     return yolosharp_b200
@@ -232,7 +232,7 @@ def test_fp16_layers_v8n(y, flags, label):
 
 @pytest.mark.parametrize("size", ["s", "x"])
 def test_fp16_layers_wide_models(y, size):
-    """v8s / v8x in tcgen05 mode, layer by layer: streamed weights with tile pairs (odd tile counts, several N tiles
+    """v8s / v8x in tensor-core mode, layer by layer: streamed weights with tile pairs (odd tile counts, several N tiles
     per layer), ragged channel slabs (80 / 160 / 400 channels), dynamic tile queue."""
     m = oracle_model("v8", "detect", size)
     x = synth_image(3, 256, 320)
@@ -270,7 +270,7 @@ def test_fp16_tcgen05_matches_cuda_core_twin(y):
 
 
 def test_fp16_detections_real_weights(y):
-    """Shipped Yolov8n weights + bus.jpg in fp16 tcgen05 mode: same detections as the fp32 oracle
+    """Shipped Yolov8n weights + bus.jpg in fp16 tensor-core mode: same detections as the fp32 oracle
     (classes equal, boxes within 2 px, scores within 0.02)."""
     m, sd = oracle_real_v8n()
     img = torch.from_numpy(np.load(os.path.join(GOLDEN, "bus_u8.npy")))
@@ -289,7 +289,7 @@ def test_fp16_detections_real_weights(y):
 
 
 def test_fp16_detections_640(y):
-    """configs[1] shape (batch of 640x640, fp16 tcgen05), synthetic weights: the prediction tensor stays
+    """configs[1] shape (batch of 640x640, fp16 tensor-core), synthetic weights: the prediction tensor stays
     within fp16 tolerance of the fp32 oracle and the strong detections survive.  (Random weights give
     heavily overlapping boxes whose near-threshold NMS decisions flip under fp16 noise, hence the
     loose survival bound; exact NMS behaviour is covered by the bit-exact NMS tests.)"""

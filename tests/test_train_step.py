@@ -128,8 +128,8 @@ def _compare_tc(step_cls, ops_cls, arch, head_tol):
     cos = float((gt * ga).sum() / (gt.norm() * ga.norm()))
     print(f"{arch}: head outputs rms rel box {e_box:.2e} cls {e_cls:.2e}; flat gradient rel L2 {l2:.2e} cosine {cos:.6f}")
     assert e_box < head_tol and e_cls < head_tol
-    # observed on B200: v8 rel L2 0.13 / cosine 0.992, v11 0.21 / 0.977; PyTorch's own cuDNN TF32 convolutions against its
-    # fp32 ones on the same model and batch: tools/exp_torch_tf32.py (profiles/r2_exp_torch_tf32.txt)
+    # PyTorch's own cuDNN TF32 convolutions against its fp32 ones on the same model and batch differ by the same order
+    # (tools/exp_torch_tf32.py)
     assert l2 < 0.4 and cos > 0.93  # a chaotic quantity: one last-bit reordering anywhere moves it by a few percent
     c = step_cls(sd0, "n", 80, device="cuda", ops=ops_cls(tensor_cores=True), lr=1e-3)
     it_tc = c.step(x, targets).cpu()
@@ -138,7 +138,7 @@ def _compare_tc(step_cls, ops_cls, arch, head_tol):
 
 @pytest.mark.gpu
 def test_train_step_tensor_cores_gpu():
-    """Every dense convolution (forward, dgrad, wgrad) on the TF32 tcgen05 kernels - the default of KernelOps, the
+    """Every dense convolution (forward, dgrad, wgrad) on the TF32 tensor-core kernels - the default of KernelOps, the
     arithmetic class of libtorch's own CUDA convolutions."""
     import yolosharp_b200  # noqa: F401
     from yolosharp_b200.train import KernelOps, TrainStepV8
@@ -276,7 +276,7 @@ def test_train_step_v11_kernels_gpu():
 
 @pytest.mark.gpu
 def test_train_step_v11_tensor_cores_gpu():
-    """YOLOv11n step with the dense convolutions on the TF32 tcgen05 kernels (depthwise conv / attention stay fp32)."""
+    """YOLOv11n step with the dense convolutions on the TF32 tensor-core kernels (depthwise conv / attention stay fp32)."""
     import yolosharp_b200  # noqa: F401
     from yolosharp_b200.train_v11 import KernelOpsV11, TrainStepV11
     _compare_tc(TrainStepV11, KernelOpsV11, "v11", 1e-1)

@@ -14,6 +14,22 @@ from oracle import modules as om  # noqa: E402
 from oracle import yolo as oyolo  # noqa: E402
 
 
+def shipped_checkpoint(name, directory):
+    """The reference's shipped checkpoint `name` (Assets/PreTrainedModels/), rebuilt byte for byte in `directory` from its
+    golden tensors, which are stored in file order with their dtypes; the file's SHA-256 is checked against the one recorded
+    from the original (tests/golden/shipped_checkpoints.json).  Returns the path."""
+    import hashlib
+    import json
+    from yolosharp_b200 import binfmt  # the host-side writer (pure Python)
+    meta = json.load(open(os.path.join(GOLDEN, "shipped_checkpoints.json")))[name]
+    z = np.load(os.path.join(GOLDEN, meta["golden"]))
+    code = {np.dtype(np.float16): 5, np.dtype(np.float32): 6}
+    path = os.path.join(str(directory), name)
+    binfmt.write_bin(path, [(k, code[z[k].dtype], list(z[k].shape), z[k].tobytes()) for k in z.files])
+    assert hashlib.sha256(open(path, "rb").read()).hexdigest() == meta["sha256"], name
+    return path
+
+
 def nms_case(seed, B, nc, A, extra=0, score_scale=1.0, quant=None, frac=1.0):
     """Same generator as tests/golden/make_golden.py (kept in sync by test_oracle.py)."""
     g = torch.Generator().manual_seed(seed)

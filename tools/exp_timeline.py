@@ -1,5 +1,5 @@
-"""Timeline of one tcgen05 conv launch (CTA 0): per tile, cycles relative to the first stamp.
-cols: MMA[start, got_tempty, got_fullA, issued+committed]  EPI[start_wait, got_tfull, done]"""
+"""Timeline of one tensor-core conv launch (CTA 0): per tile, cycles relative to the first stamp.
+cols (thread 0 of the first consumer warpgroup): [tile start, accumulator complete (main loop done), epilogue done]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ctypes as C
@@ -23,4 +23,4 @@ for idx in [int(a) for a in sys.argv[1:]] or [44]:
     print(f"--- conv_tc launch #{idx}")
     for i in range(16):
         if int(t[i, 0]) == 0: break
-        print(i, [int(v) - t0 if int(v) else 0 for v in t[i, :7]])
+        print(i, [int(t[i, k]) - t0 if int(t[i, k]) else 0 for k in (0, 3, 6)])

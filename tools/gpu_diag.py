@@ -1,4 +1,4 @@
-"""First-contact diagnostics on a real B200 (not a test: prints per-op errors, never asserts).
+"""First-contact diagnostics on a real H100 (not a test: prints per-op errors, never asserts).
 Each section runs in its own subprocess so that a trapped kernel (sticky CUDA error) cannot take
 the other sections down.   python tools/gpu_diag.py [section ...]"""
 import os
@@ -102,7 +102,7 @@ def sec_f16tc():
     e = y.Engine("v8", "n", "detect", 80, "f16", 0, 2, 256, 320, flags=2)
     e.load_state_dict(m.state_dict())
     e.finalize()
-    per_op_report(e, m, x, x.cuda(), "f16-tcgen05", ref_engine=ref)
+    per_op_report(e, m, x, x.cuda(), "f16-tc", ref_engine=ref)
 
 
 def sec_f16tc_s():
@@ -117,7 +117,7 @@ def sec_f16tc_s():
     e = y.Engine("v8", "s", "detect", 80, "f16", 0, 1, 256, 320, flags=2)
     e.load_state_dict(m.state_dict())
     e.finalize()
-    per_op_report(e, m, x, x.cuda(), "f16-tcgen05-s", ref_engine=ref)
+    per_op_report(e, m, x, x.cuda(), "f16-tc-s", ref_engine=ref)
 
 
 def sec_time():

@@ -1,6 +1,6 @@
 """Per-op device times of one eager forward (CUDA events around every launch) with the
 algorithmic bytes/FLOPs of each op and the fraction of its own roofline bound.
-    python tools/profile_ops.py [v8n|v8s|v8x] [batch] > profiles/ops_<model>.txt"""
+    python tools/profile_ops.py [v8n|v8s|v8x] [batch] > ops_<model>.txt"""
 import json
 import os
 import sys

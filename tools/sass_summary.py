@@ -1,5 +1,5 @@
-"""Opcode census of the shipped library: per kernel, how many tcgen05 / TMA / mbarrier instructions its SASS holds
-(`cuobjdump -sass yolosharp_b200/lib/libyolob200.so`).  python tools/sass_summary.py > profiles/r2_sass_opcodes.txt"""
+"""Opcode census of the shipped library: per kernel, how many wgmma / mma.sync / TMA / mbarrier instructions its SASS
+holds (`cuobjdump -sass yolosharp_b200/lib/libyolob200.so`).  python tools/sass_summary.py"""
 import collections
 import os
 import re
@@ -9,7 +9,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 so = os.path.join(ROOT, "yolosharp_b200", "lib", "libyolob200.so")
 out = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True, check=True).stdout
-WATCH = ["UTCHMMA", "UTCQMMA", "UTCMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "UTCCP", "SYNCS", "ELECT", "HMMA", "IMMA",
+WATCH = ["HGMMA", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "UTCCP", "SYNCS", "ELECT", "HMMA", "IMMA",
          "FFMA", "HFMA2", "MUFU", "LDG", "STG", "LDS", "STS", "ATOM", "RED", "SHFL", "BAR"]
 per = collections.OrderedDict()
 cur = None
@@ -38,12 +38,11 @@ for c in per.values():
     tot.update(c)
 print(f"# {os.path.relpath(so, ROOT)}: arch {sorted(arch)}, {len(per)} kernels, {tot['_total']} SASS instructions")
 print("# whole library: " + "  ".join(f"{w} {tot[w]}" for w in WATCH if tot[w]))
-print("# kernels that use the tensor cores / TMA / tensor memory:")
-cols = ["UTCHMMA", "UTCQMMA", "UTCMMA", "LDTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "SYNCS", "ELECT"]
+print("# kernels that use the tensor cores / TMA:")
+cols = ["HGMMA", "HMMA", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS"]
 print(f"{'kernel':58s} " + " ".join(f"{c:>8s}" for c in cols) + "    total")
 for name, c in per.items():
-    if any(c[k] for k in cols[:8]):
+    if any(c[k] for k in cols[:5]):
         print(f"{name[:58]:58s} " + " ".join(f"{c[k]:8d}" for k in cols) + f" {c['_total']:8d}")
-print("# (UTCHMMA = tcgen05.mma kind::f16 / tf32, LDTM = tcgen05.ld, UTMALDG = cp.async.bulk.tensor load, UBLKCP = cp.async.bulk,")
-print("#  UTCBAR = tcgen05.commit -> mbarrier, SYNCS = mbarrier try_wait / arrive; no HMMA / IMMA (mma.sync) instruction in the library:")
-print(f"#  HMMA {tot['HMMA']}, IMMA {tot['IMMA']})")
+print("# (HGMMA = wgmma.mma_async, HMMA = mma.sync (TF32 weight gradient), UTMALDG = cp.async.bulk.tensor load,")
+print("#  UBLKCP = cp.async.bulk, SYNCS = mbarrier try_wait / arrive)")

@@ -1,4 +1,4 @@
-"""yolosharp_b200: B200-native (sm_100a) YOLO forward + NMS engine behind the YoloSharp interface.
+"""yolosharp_b200: H100-native (sm_90a) YOLO forward + NMS engine behind the YoloSharp interface.
 
 The product is the C-ABI shared library `lib/libyolob200.so` (sources in `csrc/`, header in
 `include/yolob200.h`); this package is its host-side mirror of the reference's operator surface.

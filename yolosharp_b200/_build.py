@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library (nvcc, sm_100a only) in-tree: yolosharp_b200/lib/libyolob200.so."""
+"""Build the C-ABI shared library (nvcc, sm_90a only) in-tree: yolosharp_b200/lib/libyolob200.so."""
 import os
 import shutil
 import subprocess
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libyolob200.so")
 SOURCES = ["engine.cu", "kernels_generic.cu", "nms.cu", "conv_tc.cu", "loss.cu", "bn_train.cu", "comm.cu", "train_v11.cu", "ckpt.cu", "val.cu", "conv_tf32.cu", "topk.cu", "heads.cu", "train_step.cu", "metrics.cu", "segloss.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 
@@ -29,7 +29,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a into one shared library. Returns its path."""
+    """Compile every CUDA source for sm_90a into one shared library. Returns its path."""
     if not force and not needs_build():
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)

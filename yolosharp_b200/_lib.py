@@ -135,7 +135,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise ImportError(f"{LIB_PATH} is missing - run `python -c 'import __graft_entry__ as g; g.build()'` "
-                              "(nvcc, sm_100a). yolosharp_b200 has no CPU fallback.")
+                              "(nvcc, sm_90a). yolosharp_b200 has no CPU fallback.")
         l = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(l, name)  # AttributeError if the symbol is not exported

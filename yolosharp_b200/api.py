@@ -11,7 +11,7 @@ and error behaviour), implemented on the C ABI of libyolob200.so:
   Types/YoloResult.cs  YoloResult                              YoloResult
   Data/Config.cs       Config (fields used by the path)        Config
 
-There is no CPU implementation here: constructing any of these without a B200 raises.
+There is no CPU implementation here: constructing any of these without an H100 raises.
 """
 from dataclasses import dataclass, field
 from typing import List, Optional
@@ -54,7 +54,7 @@ class Config:
     ImageSize: int = 640
     PredictThreshold: float = 0.3
     IouThreshold: float = 0.7
-    ScalarType: str = "Float16"      # Float16 -> tcgen05 throughput mode, Float32 -> parity mode
+    ScalarType: str = "Float16"      # Float16 -> tensor-core throughput mode, Float32 -> parity mode
     DeviceIndex: int = 0
     End2End: bool = False            # reference default is true (Config.cs:239); the NMS path needs false
     MaxBatch: int = 1

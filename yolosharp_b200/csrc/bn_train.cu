@@ -22,7 +22,7 @@ namespace {
 
 constexpr int BN_TX = 32, BN_TY = 8, BN_ROWS_PER_BLOCK = 256, BN_MAX_SLABS = 512;
 // rows per slab: 256, or more for tall matrices so that the serial fold of the per-slab partials (bn_finish_kernel, one
-// thread per channel) stays <= 512 steps (the 1.6 M-row first layers had 6 400 slabs: 16 us per fold, 243 folds a step)
+// thread per channel) stays <= 512 steps (the 1.6 M-row first layers would otherwise have 6 400 slabs)
 static int bn_rows_per_block(long long M) {
   const long long r = (M + BN_MAX_SLABS - 1) / BN_MAX_SLABS;
   return (int)std::max<long long>(BN_ROWS_PER_BLOCK, (r + BN_TY - 1) / BN_TY * BN_TY);
@@ -82,12 +82,11 @@ __global__ void __launch_bounds__(BN_TX* BN_TY) bn_partial_kernel(int mode, int 
   }
 }
 
-// (A 4-channels-per-thread variant with 16-byte loads was no faster: 3.5 vs 3.1 ms over the 162 launches of a YOLOv11s step -
-// the kernel is bound by rows in flight, not by load width.)
+// (The kernel is bound by rows in flight, not by load width.)
 // fold the per-slab partials in a FIXED order; step 0 -> mean, step 1 -> var / invstd / running stats, step 2 -> dgamma,
 // dbeta, step 3 -> mean / var from shifted sums.  Block = 32 channels x 8 lanes: lane y sums slabs y, y+8, ... in order,
-// the 8 partial sums are then added in lane order (one thread per channel walking 512 slabs serially took 12 us per fold,
-// 243 folds a step).
+// the 8 partial sums are then added in lane order (one thread per channel walking 512 slabs serially would be a long
+// dependent-load chain).
 __global__ void __launch_bounds__(256) bn_finish_kernel(int step, const float* __restrict__ p0, const float* __restrict__ p1, int slabs, int C,
                                  long long M, float eps, float momentum, float* __restrict__ mean, float* __restrict__ invstd,
                                  float* __restrict__ running_mean, float* __restrict__ running_var, float* __restrict__ dgamma,
@@ -153,8 +152,8 @@ struct BnStat {
 };
 
 // rows per batch: 8 x 16 B (forward, z only) / 2 x 2 x 16 B (backward, z and dy) in flight per thread.  The backward pass
-// is instruction-bound (SiLU' = exp + two divisions per element: ncu issue-active 56 % at 32 % occupancy with an 80-register
-// batch of 4, profiles/r2_ncu_bn_kernels.txt): a batch of 2 fits 64 registers = 4 CTAs per SM
+// is instruction-bound (SiLU' = exp + two divisions per element), so occupancy matters more than loads in flight: a batch
+// of 2 fits 64 registers = 4 CTAs per SM
 constexpr int BN4_U_FWD = 8, BN4_U_BWD = 2;
 
 template <int MODE>  // 3: forward shifted sums (S1, S2 about K = z[row 0]); 2: backward sums (sum g, sum g * xhat)
@@ -251,8 +250,7 @@ __global__ void __launch_bounds__(256, 4) bn_stats4_kernel(const BnStat a) {
   // the last block of this channel column: fold the slabs (lane y takes slabs y, y + LY, ... in order; lanes added in order)
   float4 q0 = make_float4(0.f, 0.f, 0.f, 0.f), q1 = q0;
   if (on) {
-    // 4 slabs per batch, loads first (L2 latency ~0.4 us per dependent step: a one-load-at-a-time walk over 100 slabs per
-    // lane set the 8 us floor of the small layers)
+    // 4 slabs per batch, loads first (a one-load-at-a-time walk over 100 slabs per lane pays the L2 latency 100 times)
     const int mine = a.slabs > ty ? (a.slabs - ty + LY - 1) / LY : 0;
     const float* f0 = a.p0 + (size_t)ty * a.C + c;
     const float* f1 = a.p1 + (size_t)ty * a.C + c;
@@ -361,8 +359,7 @@ __global__ void bn_silu_dz_kernel(const float* __restrict__ z, const float* __re
 
 // Elementwise passes, 4 channels per thread: a thread owns one channel quad and walks rows r0 + ty, + LY, ... of its slab, so
 // the per-channel vectors (mean, invstd, gamma, beta [, dgamma, dbeta]) are loaded ONCE per thread instead of once per
-// element and there is no index division.  (One float4 per thread with the parameters re-loaded per element ran at 69 - 73 %
-// issue-active and 53 - 59 % of the DRAM rate on the 160 x 160 layers, profiles/r2_ncu_bn_kernels.txt.)
+// element and there is no index division.
 struct BnRows {
   const float *z, *dy;
   float* out;
@@ -585,7 +582,7 @@ int adamw_step(float* p, const float* g, float* m, float* v, long long n, int st
 
 // ------------------------------------------------------------------------------------------
 // Convolution backward, fp32 CUDA-core parity path (the training-side twin of conv_generic_kernel: correct and
-// deterministic first; the tcgen05 dgrad / wgrad kernels of the throughput path will be checked against it).
+// deterministic first; the tensor-core dgrad / wgrad kernels of the throughput path will be checked against it).
 //   dz (N, Ho, Wo, Cout) NHWC, weights in the reference's checkpoint layout (Cout, Cin, k, k)
 //   dgrad  dx[n,h,w,ci] = sum_{kh,kw,co} dz[n,(h+pad-kh)/s,(w+pad-kw)/s,co] * W[co,ci,kh,kw]   (only exact divisions)
 //   wgrad  dW[co,ci,kh,kw] = sum_{n,ho,wo} dz[n,ho,wo,co] * x[n,ho*s+kh-pad,wo*s+kw-pad,ci]

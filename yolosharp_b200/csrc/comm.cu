@@ -4,8 +4,7 @@
 // Design target: SURVEY.md section 8(e) - "forward + NMS locally into fixed-capacity (B_local, 300, 6[+32]) +
 // counts buffers, then one all-gather so every rank holds all detections in image order".  The reference has no
 // counterpart (Data/Config.cs:301: single device).  ncclAllGather is a rendezvous: its kernel must be co-resident
-// on all ranks to make progress, and on a GPU whose SMs are held by persistent forward kernels it starves (round 1:
-// 5 ms per step at 8 ranks for a 1.8 MB exchange).  Here every rank PUSHES its payload into a window of every peer
+// on all ranks to make progress, and on a GPU whose SMs are held by persistent forward kernels it starves.  Here every rank PUSHES its payload into a window of every peer
 // with plain stores through peer-mapped pointers (cudaIpc), then publishes a sequence number per (slot, source);
 // consumers poll flags in their OWN memory.  No rank ever waits inside a kernel for a peer's kernel to be scheduled
 // at the same time.

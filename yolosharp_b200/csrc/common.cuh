@@ -1,4 +1,4 @@
-// Shared declarations for the yolob200 engine (sm_100a only).
+// Shared declarations for the yolob200 engine (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -22,7 +22,7 @@ struct View {
 
 enum Act { ACT_NONE = 0, ACT_SILU = 1 };
 
-// Head-tail fusion (tcgen05 path): the final 1x1 convs of the Detect branches write straight into the
+// Head-tail fusion (tensor-core path): the final 1x1 convs of the Detect branches write straight into the
 // prediction tensor (B, Ctot, A) instead of an NHWC buffer (Modules/Head.cs:204-223 decode).
 enum EpiMode { EPI_STORE = 0, EPI_DFL_BOX = 1, EPI_SIGMOID = 2, EPI_RAW = 3 };
 struct EpiDecode {
@@ -62,14 +62,14 @@ void set_error(const std::string& msg);
 
 // ---- programmatic dependent launch for the kernels of the training step ----
 // A kernel launched through launch_pdl may be scheduled while its predecessor in the stream is still running: its CTAs
-// become resident as the predecessor's retire, run their prologue (parameter loads, barrier / TMEM setup, descriptor
+// become resident as the predecessor's retire, run their prologue (parameter loads, barrier setup, descriptor
 // prefetch) and block in pdl_wait() until the predecessor has completed and its writes are visible.  Every such kernel
 // calls pdl_wait() before its first global-memory access and pdl_trigger() right AFTER it: the successor can be scheduled
 // once all CTAs of this kernel have passed their wait, so at most two kernels of the chain are ever in flight (this one
 // finishing, the next one in its prologue).  (Triggering before the wait lets a whole chain of small kernels become
 // resident at once; with that form a seven-kernel loss chain read a scalar before its producer's atomics - not understood,
-// so the conservative order is used everywhere.)  A dependent step of ~800 small kernels otherwise pays ~1.8 us of drain +
-// launch + fill per boundary (profiles/r2_train_profile_v11s_native.txt: 16.8 ms of kernels in an 18.2 ms step).
+// so the conservative order is used everywhere.)  A dependent step of ~800 small kernels otherwise pays a drain + launch +
+// fill at every boundary.
 // Both instructions are no-ops in a kernel launched the ordinary way, so a kernel may be launched either way.
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -142,7 +142,7 @@ bool attention_tiled_32x64_fits(int N);
 template <typename T>
 int launch_proto_out(const View& in, float* out, int B, cudaStream_t s);
 
-// ---- conv_tc.cu : tcgen05 implicit-GEMM conv (fp16 storage, fp32 accumulate in TMEM) ----
+// ---- conv_tc.cu : wgmma implicit-GEMM conv (fp16 storage, fp32 accumulate) ----
 struct TcConvPlan;  // opaque: tensor maps + tiling for one conv layer
 TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err);
 void tc_conv_plan_destroy(TcConvPlan* plan);

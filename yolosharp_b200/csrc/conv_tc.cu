@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM convolution for sm_100a (fp16 NHWC activations, fp32 accumulate in TMEM).
+// wgmma implicit-GEMM convolution for sm_90a (fp16 NHWC activations, fp32 accumulate in registers).
 //
 // Computes the reference's Conv block (Modules/Convs.cs:36-56: Conv2d -> BatchNorm2d -> SiLU, BN
 // folded into weights/bias at load) and the Bottleneck shortcut (Block.cs:606) as ONE kernel:
@@ -11,13 +11,13 @@
 //               (= conv zero padding), stride-2 convs use the tensor map's traversal stride
 //   B operand   weights [Cout][tap][Cin] fp16, 2-D TMA box {BK, n_tile}
 //   swizzle     BK = 64/32/16 channels -> SWIZZLE_128B/64B/32B rows, identical in the TMA map and
-//               the UMMA shared-memory descriptors
-//   MMA         tcgen05.mma.cta_group::1.kind::f16, M=128, N=n_tile, K=16 per instruction, issued
-//               by one thread; accumulators double-buffered in TMEM (2 x n_tile columns)
-//   epilogue    4 warps: tcgen05.ld (32 lanes x 16 columns) -> +bias -> SiLU -> +residual -> fp16 ->
-//               16-byte stores into the channel slice of the (concat) output buffer
-//   schedule    persistent CTAs (one per SM), warp-specialised: warp0 = TMA producer, warp1 = MMA
-//               issuer (+TMEM alloc), warps2-5 = epilogue; smem ring of `stages` slabs.
+//               the wgmma shared-memory descriptors
+//   MMA         wgmma.mma_async m64nNk16 f16 -> f32: two consumer warpgroups, each owning 64 rows of the
+//               tile and its n_tile accumulator columns in registers
+//   epilogue    the same warpgroups: +bias -> SiLU -> +residual -> fp16 stores into the channel slice of
+//               the (concat) output buffer
+//   schedule    persistent CTAs (one or two per SM), warp-specialised: warps 0-7 = consumers, warp 8 = TMA
+//               producer; smem rings of `stages` slabs the producer fills ahead of the consumers.
 #include <cuda.h>
 
 #include <algorithm>
@@ -57,16 +57,11 @@ struct TcArgs {
   int stages_a, stages_b;
   uint32_t a_bytes, b_bytes;      // TMA transaction bytes per A slab / B slab
   uint32_t a_stride, b_stride;    // smem bytes reserved per slab (1 KiB aligned)
-  uint32_t sbo_a, sbo_b;          // UMMA stride-byte-offset between 8-row groups, >> 4
+  uint32_t sbo_a, sbo_b;          // wgmma stride-byte-offset between 8-row groups, >> 4
   uint32_t row_bytes;             // BK * 2
-  uint32_t layout_a, layout_b;    // UMMA LayoutType: 2 = SW128, 4 = SW64, 6 = SW32
-  uint32_t tmem_cols;
-  int n_issuers;                  // 1 or 2 MMA-issuing warps (each with its own half of the rings)
-  int n_groups;                   // epilogue groups of 4 warps (2 or 4)
-  int n_acc;                      // TMEM accumulator buffers (2 or 4)
+  uint32_t layout_a, layout_b;    // wgmma layout type: 1 = SW128, 2 = SW64, 3 = SW32
   int total_tiles;
   int b_resident;                 // all weight slabs stay in smem for the CTA's lifetime
-  int dual;                       // streamed weights: tiles are processed in pairs that share every weight slab
   int ksteps;
   // fused head decode (EpiDecode)
   int epi_mode, dA, dCtot, da0, dch0, dWl, dHW;
@@ -89,11 +84,11 @@ struct TcConvPlan {
   ConvParams p;
   bool flat;   // 1x1 stride-1 conv on the flattened pixel dimension
   int occ;     // CTAs per SM this plan is sized for
-  int threads; // 3 role warps + 4 warps per epilogue group
   bool small;  // <= 2 tiles per CTA
   size_t smem;
   int grid;
   uint8_t* wpk = nullptr;  // device, owned: packed weight slabs
+  void (*kernel)(TcArgs) = nullptr;  // conv_tc_kernel<n_tile / 16>
 };
 
 __device__ __forceinline__ int fdiv(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
@@ -107,28 +102,20 @@ __device__ __forceinline__ float silu_tanh(float v) {
   return fmaf(h, t, h);
 }
 
-constexpr int TC_MAX_THREADS = 608;  // warp 0 TMA producer, warps 1-2 MMA issuers, warps 3.. epilogue groups of 4 warps
-constexpr int TC_MAX_GROUPS = 4;
-constexpr int TC_ISSUERS = 2;
-constexpr int TC_MAX_ACC = 4;
+constexpr int TC_CONSUMERS = 256;                // warps 0-7: two warpgroups, rows 0-63 / 64-127 of every tile
+constexpr int TC_THREADS = TC_CONSUMERS + 32;    // warp 8: TMA producer
+constexpr int TC_CONSUMER_WARPS = TC_CONSUMERS / 32;
 constexpr int TC_MAX_COUT = 1024;
 constexpr int TC_MAX_STAGES = 12;
 constexpr int HALO_BW = 8, HALO_BH = 16;  // output rectangle of a halo tile (128 rows)
 
 // ------------------------------------------------------------------------------------------
-// MMA issue loop.  One thread issues every tcgen05.mma of the CTA, so its per-instruction overhead is
-// the kernel's pace for small N (a 128x64x16 MMA occupies the tensor pipe for ~34 cycles; the measured
-// single-thread issue floor is ~55 cycles, tools/exp_mma_issue.cu).  Everything that can be hoisted is
-// hoisted: descriptor high words are loop constants, low words advance by compile-time amounts
-// (KK = BK/16 MMAs per slab, tap shifts of the halo tile), kernel parameters live in registers.
-// ------------------------------------------------------------------------------------------
-// ------------------------------------------------------------------------------------------
 // Dynamic tile scheduler.  The producer thread draws tile indices from a global counter (first tile =
-// blockIdx.x, then gridDim.x + atomicAdd) and publishes them in a small shared-memory queue that the MMA
-// issuers and epilogue groups follow.  CTAs that start late - SMs held by a concurrent kernel (NMS of the
-// previous batch, a sibling head branch) - simply take fewer tiles instead of delaying the whole grid with a
-// fixed share.  The queue cannot wrap onto unread entries: the producer is at most stages_a + n_acc + groups
-// (< 32) tiles ahead of the slowest reader.
+// blockIdx.x, then gridDim.x + atomicAdd) and publishes them in a small shared-memory queue that the consumer
+// warpgroups follow.  CTAs that start late - SMs held by a concurrent kernel (NMS of the previous batch, a sibling
+// head branch) - simply take fewer tiles instead of delaying the whole grid with a fixed share.  The queue cannot
+// wrap onto unread entries: every tile takes at least one ring slot, so the producer is at most stages_a (< 32)
+// tiles ahead of the consumers.
 // ------------------------------------------------------------------------------------------
 constexpr int TQ = 32;
 __device__ __forceinline__ void tq_publish(int* s_tile, volatile int* s_head, int li, int tile) {
@@ -157,256 +144,237 @@ __device__ __forceinline__ void dep_wait_image(const int* ctr, int img, int expe
   }
 }
 
-__device__ __forceinline__ uint64_t desc64(uint32_t lo, uint32_t hi) {
-  uint64_t d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
-  return d;
-}
-
-// Residual (Bottleneck shortcut) values of this lane's own row for one 32/16-column block, issued BEFORE
-// the accumulator is awaited so the global-load latency overlaps the MMAs.
-__device__ __forceinline__ void res_prefetch(const TcArgs& a, int n0, int cb0, size_t pix, bool valid, int4 (&rv)[4]) {
-  const int wb = min(32, a.n_tile - cb0);
-  const __half* rrow = a.res + pix * a.res_pitch + a.res_coff + n0 + cb0;
-#pragma unroll
-  for (int g = 0; g < 4; g++) {
-    rv[g] = make_int4(0, 0, 0, 0);
-    // L2-only load: with layer chaining a neighbouring row of the same 128-byte line may still be unwritten when
-    // this one is read, and a line cached in L1 now would be stale when that row's own tile reads it later
-    if (valid && g * 8 < wb) rv[g] = __ldcg(reinterpret_cast<const int4*>(rrow + g * 8));
-  }
-}
-
-// every lane of the issuing warp waits; the warp is converged again before the next elect.sync
-__device__ __forceinline__ void mbar_wait_warp(uint32_t bar, uint32_t parity) {
-  mbar_wait(bar, parity);
-  __syncwarp();
-}
-
-template <int KK>
-__device__ __forceinline__ void mma_role(const TcArgs& a, uint32_t smemA, uint32_t smemB, uint32_t tmem_base,
-                                         uint32_t fullA, uint32_t emptyA, uint32_t fullB, uint32_t emptyB,
-                                         uint32_t tfull0, uint32_t tempty0, uint32_t bfull, int issuer,
-                                         const int* s_tile, const volatile int* s_head) {
-  const uint32_t n_tile = a.n_tile;
-  const uint32_t idesc = (1u << 4) | ((n_tile >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  // descriptor = lo | hi << 32 :  lo = start>>4 | LBO(1)<<16 ;  hi = SBO | version(1)<<14 | layout<<29
-  const uint32_t a_hi = a.sbo_a | (1u << 14) | (a.layout_a << 29);
-  const uint32_t b_hi = a.sbo_b | (1u << 14) | (a.layout_b << 29);
-  const uint32_t lo_flags = 1u << 16;
-  const uint32_t a_stride16 = a.a_stride >> 4, b_stride16 = a.b_stride >> 4;
-  const uint32_t a_lo0 = ((smemA & 0x3FFFF) >> 4) | lo_flags, b_lo0 = ((smemB & 0x3FFFF) >> 4) | lo_flags;
-  const int stages_a = a.stages_a, stages_b = a.stages_b, chunks = a.chunks, ksteps = a.ksteps;
+// ------------------------------------------------------------------------------------------
+// Main loop of one tile for one consumer warpgroup (its 64 rows of the 128-row tile, all n_tile columns).
+// Every K step is one wgmma commit group; after issuing group g the warpgroup waits for group g-1 and frees the ring
+// slots g-1 read (one arrive per warp: the empty barriers count 8), so the tensor pipe always has the next group
+// queued while a slot is handed back to the producer.
+//   TC_TAP  - one 128-row A slab per (tap, channel slab)
+//   TC_HALO - one (BH+2)x(BW+2)-pixel halo tile per channel slab; the 9 taps of a 3x3 stride-1 conv are issued from
+//             the SAME bytes with the descriptor start shifted by (kh*(BW+2)+kw) rows and SBO = (BW+2) rows (the
+//             swizzle follows absolute address bits, tc_ptx.cuh) -> 180 TMA rows per slab instead of 9 x 128
+//   TC_S2P  - stride-2 pair rows, the same idea with (input row, pair, half) shifts
+// B: one [n_tile x BK] weight slab per (tap, channel slab), streamed through its own ring or all resident.
+// ------------------------------------------------------------------------------------------
+template <int NT16, int KK>
+__device__ __forceinline__ void tc_mainloop(const TcArgs& a, float* acc, int wg, uint32_t smemA, uint32_t smemB, uint32_t fullA,
+                                            uint32_t emptyA, uint32_t fullB, uint32_t emptyB, int& sa, uint32_t& pa, int& sb,
+                                            uint32_t& pb) {
   const bool resident = a.b_resident != 0, halo = a.mode != TC_TAP, s2p = a.mode == TC_S2P;
-  const int total_tiles = a.total_tiles, gstride = gridDim.x;
-  constexpr uint32_t ROW16 = KK * 2;  // bytes per operand row / 16
-  // Two issuer warps take alternate tiles (local tile index li = issuer, issuer+2, ...): one thread tops
-  // out at ~55-80 cycles per tcgen05.mma, two keep the tensor pipe fed for N <= 64.  Each issuer owns its
-  // own half of the A (and B) ring - the producer fills ring (li % n_issuers) for tile li - so every
-  // mbarrier is waited on strictly in phase order by exactly one thread (a parity wait cannot tell
-  // "two phases behind" from "done").
-  const int nb = a.n_acc;                      // TMEM accumulator buffers
-  const int ni = a.n_issuers;
-  if (issuer >= ni) return;
-  const int ra = stages_a / ni, rb = resident ? 0 : stages_b / ni;  // ring depth per issuer
-  const int a_base = issuer * ra, b_base = issuer * rb;
-  int sa = 0, sb = 0;
-  uint32_t pa = 0, pb = 0;
-  if (resident) mbar_wait_warp(bfull, 0);
-  const bool dyn = a.tile_ctr != nullptr;
-  for (int li = issuer;; li += ni) {
-    const int tile = dyn ? tq_get(s_tile, s_head, li) : (int)blockIdx.x + li * gstride;
-    __syncwarp();
-    if (tile < 0 || tile >= total_tiles) break;
-    const int dbg_i = li;
-    const int acc = li & (nb - 1);  // nb is 2 or 4
-    const uint32_t aphase = (uint32_t)(li >> (nb == 4 ? 2 : 1)) & 1u;
-    if (a.dbg && blockIdx.x == 0 && (threadIdx.x & 31) == 0 && dbg_i < 16) a.dbg[dbg_i * 8 + 0] = clock64();
-    mbar_wait_warp(tempty0 + 8 * acc, aphase ^ 1);
-    tc_fence_after();
-    if (a.dbg && blockIdx.x == 0 && (threadIdx.x & 31) == 0 && dbg_i < 16) a.dbg[dbg_i * 8 + 1] = clock64();
-    const uint32_t d_tmem = tmem_base + acc * n_tile;
-    uint32_t accf = 0;
-    if (halo) {
-      for (int ch = 0; ch < chunks; ch++) {
-        mbar_wait_warp(fullA + 8 * (a_base + sa), pa);
-        tc_fence_after();
-        if (a.dbg && blockIdx.x == 0 && (threadIdx.x & 31) == 0 && dbg_i < 16 && ch == 0) a.dbg[dbg_i * 8 + 2] = clock64();
-        const uint32_t a_lo = a_lo0 + (a_base + sa) * a_stride16;
-#pragma unroll
-        for (int t = 0; t < 9; t++) {
-          // row shift of tap t inside the staged input tile (compile-time constants after unrolling):
-          //   halo : (kh * (BW+2) + kw) pixel rows
-          //   s2p  : pair rows (input pixels 2q, 2q+1), the tile starts at pair w0-1: kw = 0 is the second half
-          //          of pair j, kw = 1 / 2 the two halves of pair j+1; kh advances one input row = (BW+1) pairs
-          const uint32_t TAP_HALO = (uint32_t)((t / 3) * (HALO_BW + 2) + (t % 3)) * ROW16;
-          const uint32_t TAP_S2P = (uint32_t)((t / 3) * (HALO_BW + 1) + (t % 3 != 0 ? 1 : 0)) * 2 * ROW16 +
-                                       (t % 3 != 1 ? ROW16 : 0);
-          const uint32_t tap16 = s2p ? TAP_S2P : TAP_HALO;
-          uint32_t b_lo;
-          if (resident) {
-            b_lo = b_lo0 + (t * chunks + ch) * b_stride16;
-          } else {
-            mbar_wait_warp(fullB + 8 * (b_base + sb), pb);
-            tc_fence_after();
-            b_lo = b_lo0 + (b_base + sb) * b_stride16;
-          }
-#pragma unroll
-          for (int k = 0; k < KK; k++) {  // +32 B per K=16 step inside the swizzled row
-            umma_f16_elect(d_tmem, desc64(a_lo + tap16 + 2 * k, a_hi), desc64(b_lo + 2 * k, b_hi), idesc, accf);
-            accf = 1;
-          }
-          if (!resident) {
-            umma_commit_elect(emptyB + 8 * (b_base + sb));
-            if (++sb == rb) { sb = 0; pb ^= 1; }
-          }
-        }
-        umma_commit_elect(emptyA + 8 * (a_base + sa));  // halo tile free once its 9 taps retired
-        if (++sa == ra) { sa = 0; pa ^= 1; }
-      }
-    } else {
-      for (int ks = 0; ks < ksteps; ks++) {
-        mbar_wait_warp(fullA + 8 * (a_base + sa), pa);
-        uint32_t b_lo;
-        if (resident) {
-          b_lo = b_lo0 + ks * b_stride16;
-        } else {
-          mbar_wait_warp(fullB + 8 * (b_base + sb), pb);
-          b_lo = b_lo0 + (b_base + sb) * b_stride16;
-        }
-        tc_fence_after();
-        const uint32_t a_lo = a_lo0 + (a_base + sa) * a_stride16;
-#pragma unroll
-        for (int k = 0; k < KK; k++) {
-          umma_f16_elect(d_tmem, desc64(a_lo + 2 * k, a_hi), desc64(b_lo + 2 * k, b_hi), idesc, accf);
-          accf = 1;
-        }
-        umma_commit_elect(emptyA + 8 * (a_base + sa));  // slab free once these MMAs retire
-        if (++sa == ra) { sa = 0; pa ^= 1; }
-        if (!resident) {
-          umma_commit_elect(emptyB + 8 * (b_base + sb));
-          if (++sb == rb) { sb = 0; pb ^= 1; }
-        }
-      }
-    }
-    umma_commit_elect(tfull0 + 8 * acc);  // accumulator complete
-    if (a.dbg && blockIdx.x == 0 && (threadIdx.x & 31) == 0 && dbg_i < 16) a.dbg[dbg_i * 8 + 3] = clock64();
-  }
-}
-
-// Streamed-weight layers (weights too large to stay resident): two tiles are accumulated side by side so that
-// every weight slab fetched from L2 feeds the MMAs of BOTH.  The timeline of a 3x3 160->160 layer (v8x) showed the
-// issuer waiting for weight slabs ~250 cycles per MMA: 148 SMs re-streaming the same 460 KB per 128-pixel tile run
-// into the L2 -> SM delivery limit, not into the tensor pipe.  One issuer (wide N: the tensor pipe is the pace).
-template <int KK>
-__device__ __forceinline__ void mma_role_dual(const TcArgs& a, uint32_t smemA, uint32_t smemB, uint32_t tmem_base,
-                                              uint32_t fullA, uint32_t emptyA, uint32_t fullB, uint32_t emptyB,
-                                              uint32_t tfull0, uint32_t tempty0) {
-  const uint32_t n_tile = a.n_tile;
-  const uint32_t idesc = (1u << 4) | ((n_tile >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  const uint32_t a_hi = a.sbo_a | (1u << 14) | (a.layout_a << 29);
-  const uint32_t b_hi = a.sbo_b | (1u << 14) | (a.layout_b << 29);
+  const uint32_t a_hi = wg_desc_hi(a.sbo_a, a.layout_a), b_hi = wg_desc_hi(a.sbo_b, a.layout_b);
   const uint32_t a_stride16 = a.a_stride >> 4, b_stride16 = a.b_stride >> 4;
-  const uint32_t a_lo0 = ((smemA & 0x3FFFF) >> 4) | (1u << 16), b_lo0 = ((smemB & 0x3FFFF) >> 4) | (1u << 16);
-  const int ra = a.stages_a, rb = a.stages_b, chunks = a.chunks, ksteps = a.ksteps, nb = a.n_acc;
-  const bool halo = a.mode != TC_TAP, s2p = a.mode == TC_S2P;
-  const int total_tiles = a.total_tiles, gstride = gridDim.x;
-  constexpr uint32_t ROW16 = KK * 2;
-  int sa = 0, sb = 0;
-  uint32_t pa = 0, pb = 0;
-  int li = 0;
-  for (int tile0 = blockIdx.x; tile0 < total_tiles; tile0 += 2 * gstride, li += 2) {
-    const int nT = (tile0 + gstride < total_tiles) ? 2 : 1;
-    uint32_t d_tmem[2] = {0, 0};
-    int acc[2] = {0, 0};
-    for (int q = 0; q < nT; q++) {
-      acc[q] = (li + q) & (nb - 1);
-      const uint32_t aphase = (uint32_t)((li + q) >> (nb == 4 ? 2 : 1)) & 1u;
-      mbar_wait_warp(tempty0 + 8 * acc[q], aphase ^ 1);
-      d_tmem[q] = tmem_base + acc[q] * n_tile;
+  const uint32_t a_lo0 = wg_desc_lo(smemA) + (uint32_t)wg * 8 * a.sbo_a;  // rows 64 * wg.. = 8 groups of 8 rows further
+  const uint32_t b_lo0 = wg_desc_lo(smemB);
+  constexpr uint32_t ROW16 = KK * 2;  // bytes per operand row / 16
+  const int ra = a.stages_a, rb = a.stages_b;
+  const bool leader = (threadIdx.x & 31) == 0;
+  uint32_t pend0 = 0, pend1 = 0;  // slots read by the previous commit group
+  uint32_t scale = 0;
+  auto step = [&](uint32_t a_lo, uint32_t b_lo, uint32_t relA, uint32_t relB) {
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < KK; k++) {  // +32 B per K=16 step inside the swizzled row
+      wg_mma_n<NT16, false>(acc, a_lo + 2 * k, a_hi, b_lo + 2 * k, b_hi, ROW16, scale);
+      scale = 1;
     }
-    tc_fence_after();
-    uint32_t alo[2] = {0, 0};
-    int stq[2] = {0, 0};
-    if (halo) {
-      for (int ch = 0; ch < chunks; ch++) {
-        for (int q = 0; q < nT; q++) {
-          mbar_wait_warp(fullA + 8 * sa, pa);
-          alo[q] = a_lo0 + sa * a_stride16;
-          stq[q] = sa;
-          if (++sa == ra) { sa = 0; pa ^= 1; }
-        }
-        tc_fence_after();
+    wg_commit();
+    wg_wait<1>();
+    __syncwarp();
+    if (leader) {
+      if (pend0) mbar_arrive(pend0);
+      if (pend1) mbar_arrive(pend1);
+    }
+    pend0 = relA;
+    pend1 = relB;
+  };
+  if (halo) {
+    for (int ch = 0; ch < a.chunks; ch++) {
+      mbar_wait(fullA + 8 * sa, pa);
+      const uint32_t a_lo = a_lo0 + sa * a_stride16;
+      const uint32_t slotA = emptyA + 8 * sa;
+      if (++sa == ra) { sa = 0; pa ^= 1; }
 #pragma unroll
-        for (int t = 0; t < 9; t++) {
-          const uint32_t TAP_HALO = (uint32_t)((t / 3) * (HALO_BW + 2) + (t % 3)) * ROW16;
-          const uint32_t TAP_S2P = (uint32_t)((t / 3) * (HALO_BW + 1) + (t % 3 != 0 ? 1 : 0)) * 2 * ROW16 +
-                                   (t % 3 != 1 ? ROW16 : 0);
-          const uint32_t tap16 = s2p ? TAP_S2P : TAP_HALO;
-          mbar_wait_warp(fullB + 8 * sb, pb);
-          tc_fence_after();
-          const uint32_t b_lo = b_lo0 + sb * b_stride16;
-          const uint32_t first = (ch == 0 && t == 0) ? 1u : 0u;
-#pragma unroll
-          for (int q = 0; q < 2; q++) {
-            if (q < nT) {
-#pragma unroll
-              for (int k = 0; k < KK; k++)
-                umma_f16_elect(d_tmem[q], desc64(alo[q] + tap16 + 2 * k, a_hi), desc64(b_lo + 2 * k, b_hi), idesc,
-                         (first && k == 0) ? 0u : 1u);
-            }
-          }
-          umma_commit_elect(emptyB + 8 * sb);
+      for (int t = 0; t < 9; t++) {
+        // row shift of tap t inside the staged input tile (compile-time constants after unrolling):
+        //   halo : (kh * (BW+2) + kw) pixel rows
+        //   s2p  : pair rows (input pixels 2q, 2q+1), the tile starts at pair w0-1: kw = 0 is the second half
+        //          of pair j, kw = 1 / 2 the two halves of pair j+1; kh advances one input row = (BW+1) pairs
+        const uint32_t TAP_HALO = (uint32_t)((t / 3) * (HALO_BW + 2) + (t % 3)) * ROW16;
+        const uint32_t TAP_S2P = (uint32_t)((t / 3) * (HALO_BW + 1) + (t % 3 != 0 ? 1 : 0)) * 2 * ROW16 +
+                                 (t % 3 != 1 ? ROW16 : 0);
+        const uint32_t tap16 = s2p ? TAP_S2P : TAP_HALO;
+        uint32_t b_lo, relB = 0;
+        if (resident) {
+          b_lo = b_lo0 + (t * a.chunks + ch) * b_stride16;
+        } else {
+          mbar_wait(fullB + 8 * sb, pb);
+          b_lo = b_lo0 + sb * b_stride16;
+          relB = emptyB + 8 * sb;
           if (++sb == rb) { sb = 0; pb ^= 1; }
         }
-        for (int q = 0; q < nT; q++) umma_commit_elect(emptyA + 8 * stq[q]);
+        step(a_lo + tap16, b_lo, t == 8 ? slotA : 0u, relB);  // halo tile free once its 9 taps retired
       }
-    } else {
-      for (int ks = 0; ks < ksteps; ks++) {
-        for (int q = 0; q < nT; q++) {
-          mbar_wait_warp(fullA + 8 * sa, pa);
-          alo[q] = a_lo0 + sa * a_stride16;
-          stq[q] = sa;
-          if (++sa == ra) { sa = 0; pa ^= 1; }
-        }
-        mbar_wait_warp(fullB + 8 * sb, pb);
-        tc_fence_after();
-        const uint32_t b_lo = b_lo0 + sb * b_stride16;
-#pragma unroll
-        for (int q = 0; q < 2; q++) {
-          if (q < nT) {
-#pragma unroll
-            for (int k = 0; k < KK; k++)
-              umma_f16_elect(d_tmem[q], desc64(alo[q] + 2 * k, a_hi), desc64(b_lo + 2 * k, b_hi), idesc,
-                       (ks == 0 && k == 0) ? 0u : 1u);
-          }
-        }
-        for (int q = 0; q < nT; q++) umma_commit_elect(emptyA + 8 * stq[q]);
-        umma_commit_elect(emptyB + 8 * sb);
+    }
+  } else {
+    for (int ks = 0; ks < a.ksteps; ks++) {
+      mbar_wait(fullA + 8 * sa, pa);
+      const uint32_t a_lo = a_lo0 + sa * a_stride16;
+      const uint32_t relA = emptyA + 8 * sa;
+      if (++sa == ra) { sa = 0; pa ^= 1; }
+      uint32_t b_lo, relB = 0;
+      if (resident) {
+        b_lo = b_lo0 + ks * b_stride16;
+      } else {
+        mbar_wait(fullB + 8 * sb, pb);
+        b_lo = b_lo0 + sb * b_stride16;
+        relB = emptyB + 8 * sb;
         if (++sb == rb) { sb = 0; pb ^= 1; }
       }
+      step(a_lo, b_lo, relA, relB);
     }
-    for (int q = 0; q < nT; q++) umma_commit_elect(tfull0 + 8 * acc[q]);  // both accumulators complete
+  }
+  wg_wait<0>();
+  __syncwarp();
+  if (leader) {
+    if (pend0) mbar_arrive(pend0);
+    if (pend1) mbar_arrive(pend1);
+  }
+  wg_fence_acc<NT16 * 8>(acc);
+}
+
+// Publish a warp's stored rows per image for the layer chain.  A publish is fence (every lane's stores before the
+// count) + warp barrier + one atomic; the fence costs several hundred cycles, so rows are counted in registers and
+// published only when the warp moves on to another image (tiles arrive in image order) or runs out of tiles.  The
+// 16 rows of a warp may span two images of a flattened tile.
+__device__ __forceinline__ void chain_count(const TcArgs& a, const bool (&valid)[2], const int (&im)[2], int& pend_img,
+                                            int& pend_cnt) {
+  const int lane = threadIdx.x & 31;
+  const bool lead = (lane & 3) == 0;  // one lane of each quad owns the quad's two rows
+  const int cand = valid[0] ? im[0] : (valid[1] ? im[1] : INT_MAX);
+  const int first = __reduce_min_sync(0xffffffffu, cand);
+  if (first == INT_MAX) return;
+  const int nall = __popc(__ballot_sync(0xffffffffu, lead && valid[0])) + __popc(__ballot_sync(0xffffffffu, lead && valid[1]));
+  const int nsame = __popc(__ballot_sync(0xffffffffu, lead && valid[0] && im[0] == first)) +
+                    __popc(__ballot_sync(0xffffffffu, lead && valid[1] && im[1] == first));
+  if (pend_img >= 0 && pend_img != first) {
+    __threadfence();
+    __syncwarp();
+    if (lane == 0) atomicAdd(a.done_ctr + pend_img, pend_cnt);
+    pend_cnt = 0;
+  }
+  pend_img = first;
+  pend_cnt += nsame;
+  if (nall != nsame) {
+    __threadfence();
+    __syncwarp();
+    if (lane == 0) atomicAdd(a.done_ctr + first, pend_cnt);
+    pend_img = first + 1;
+    pend_cnt = nall - nsame;
   }
 }
 
-// ------------------------------------------------------------------------------------------
-// Two operand rings feed the single MMA-issuing thread:
-//   A ring  : TC_TAP  - one 128-row slab per (tap, channel slab)
-//             TC_HALO - one (BH+2)x(BW+2)-pixel halo tile per channel slab; the 9 taps of a 3x3
-//                       stride-1 conv are issued from the SAME bytes with the descriptor start
-//                       shifted by (kh*(BW+2)+kw) rows and SBO = (BW+2) rows.  tcgen05 applies the
-//                       128B/64B/32B swizzle on absolute smem address bits, so a row-shifted start
-//                       needs no base-offset (verified on B200 by tools/exp_umma_shift.cu).
-//                       -> 180 TMA rows per slab instead of 9 x 128: the kernel is bound by L2
-//                       request rate (~30 requests/clk chip-wide), not by bytes.
-//   B ring  : one [n_tile x BK] weight slab per (tap, channel slab), or all slabs resident.
-// ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(704, 1) conv_tc_kernel(  // 704 = 2 x 352: caps registers at 93 so two 352-thread CTAs fit an SM
-const __grid_constant__ TcArgs a) {
+// Epilogue of one tile from the accumulator registers: +bias -> SiLU -> +residual -> fp16 into the channel slice of
+// the (concat) output buffer, or the fused Detect tail (DFL box decode / class scores into the prediction tensor).
+template <int NT16>
+__device__ __forceinline__ void tc_epilogue(const TcArgs& a, const float* acc, const float* bias, int n0, int img, int th,
+                                            int tw, int wg, bool (&valid)[2], int (&wo)[2]) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, t4 = lane & 3;
+  size_t pix[2];
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const int row = wg * 64 + (warp & 3) * 16 + g + 8 * h;
+    const int hl = fdiv(row, a.m_bw), wl = row - hl * a.BW;
+    const int ho = th * a.BH + hl;
+    wo[h] = tw * a.BW + wl;
+    valid[h] = hl < a.BH && ho < a.Ho && wo[h] < a.Wo;
+    pix[h] = ((size_t)img * a.Ho + ho) * a.Wo + wo[h];
+  }
+  if (a.epi_mode != EPI_STORE) {
+    // fused Detect tail (flattened 1x1 conv): row h of this thread is pixel wo[h] of the whole batch
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int n = valid[h] ? wo[h] / a.dHW : 0;
+      const int i = wo[h] - n * a.dHW;
+      float* po = a.pred + (size_t)n * a.dCtot * a.dA + a.da0 + i;
+      if (a.epi_mode == EPI_DFL_BOX) {
+        if constexpr (NT16 == 4) {  // tc_conv_plan_create refuses a DFL plan whose n_tile is not 64 = 4 sides x 16 bins
+          // DFL (Block.cs:44): softmax over the 16 bins of each side, expectation with weights 0..15; then
+          // dist2bbox(xywh) * stride (Tal.cs:338-356, Head.cs:221).  A quad of lanes holds the 16 bins of a side.
+          float d[4];
+#pragma unroll
+          for (int sd = 0; sd < 4; sd++) {
+            const int b0 = 2 * t4;
+            float f[4];
+            f[0] = acc[4 * (2 * sd) + 2 * h] + bias[16 * sd + b0];
+            f[1] = acc[4 * (2 * sd) + 2 * h + 1] + bias[16 * sd + b0 + 1];
+            f[2] = acc[4 * (2 * sd + 1) + 2 * h] + bias[16 * sd + 8 + b0];
+            f[3] = acc[4 * (2 * sd + 1) + 2 * h + 1] + bias[16 * sd + 9 + b0];
+            float mx = fmaxf(fmaxf(f[0], f[1]), fmaxf(f[2], f[3]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float bin[4] = {(float)b0, (float)(b0 + 1), (float)(b0 + 8), (float)(b0 + 9)};
+            float sum = 0.f, ex = 0.f;
+#pragma unroll
+            for (int j = 0; j < 4; j++) { const float e = __expf(f[j] - mx); sum += e; ex = fmaf(e, bin[j], ex); }
+            sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+            ex += __shfl_xor_sync(0xffffffffu, ex, 1);
+            sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+            ex += __shfl_xor_sync(0xffffffffu, ex, 2);
+            d[sd] = __fdividef(ex, sum);
+          }
+          if (valid[h] && t4 == 0) {
+            const int y = i / a.dWl, x = i - y * a.dWl;
+            const float ax = (float)x + 0.5f, ay = (float)y + 0.5f;
+            const float x1 = ax - d[0], y1 = ay - d[1], x2 = ax + d[2], y2 = ay + d[3];
+            po[0] = (x1 + x2) * 0.5f * a.dstride;
+            po[(size_t)a.dA] = (y1 + y2) * 0.5f * a.dstride;
+            po[(size_t)2 * a.dA] = (x2 - x1) * a.dstride;
+            po[(size_t)3 * a.dA] = (y2 - y1) * a.dstride;
+          }
+        }
+      } else if (valid[h]) {
+#pragma unroll
+        for (int J = 0; J < NT16 * 2; J++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const int c = 8 * J + 2 * t4 + e;
+            float f = acc[4 * J + 2 * h + e] + bias[c];
+            if (a.epi_mode == EPI_SIGMOID) f = __fdividef(1.0f, 1.0f + __expf(-f));
+            po[(size_t)(a.dch0 + c) * a.dA] = f;
+          }
+      }
+    }
+    return;
+  }
+  const bool use_res = a.res != nullptr;
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    if (!valid[h]) continue;
+    __half* orow = a.out + pix[h] * a.out_pitch + a.out_coff + n0;
+    const __half* rrow = use_res ? a.res + pix[h] * a.res_pitch + a.res_coff + n0 : nullptr;
+#pragma unroll
+    for (int J = 0; J < NT16 * 2; J++) {
+      const int c = 8 * J + 2 * t4;
+      const float2 b = *reinterpret_cast<const float2*>(bias + c);
+      float f0 = acc[4 * J + 2 * h] + b.x, f1 = acc[4 * J + 2 * h + 1] + b.y;
+      if (a.act == ACT_SILU) { f0 = silu_tanh(f0); f1 = silu_tanh(f1); }
+      if (use_res) {
+        // L2-only load: with layer chaining a neighbouring row of the same 128-byte line may still be unwritten when
+        // this one is read, and a line cached in L1 now would be stale when that row's own tile reads it later
+        const unsigned int rb = __ldcg(reinterpret_cast<const unsigned int*>(rrow + c));
+        const float2 x = __half22float2(*reinterpret_cast<const __half2*>(&rb));
+        f0 += x.x; f1 += x.y;
+      }
+      *reinterpret_cast<__half2*>(orow + c) = __floats2half2_rn(f0, f1);
+    }
+  }
+}
+
+template <int NT16>
+__global__ void __launch_bounds__(TC_THREADS, NT16 <= 4 ? 2 : 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
   extern __shared__ __align__(1024) uint8_t tc_smem[];
-  __shared__ __align__(8) uint64_t bars[4 * TC_MAX_STAGES + 2 * TC_MAX_ACC + 1];
-  __shared__ uint32_t tmem_base_slot;
+  __shared__ __align__(8) uint64_t bars[4 * TC_MAX_STAGES + 1];
   __shared__ int s_tile[TQ];
   __shared__ volatile int s_head;
   __shared__ __align__(16) float s_bias[TC_MAX_COUT];
@@ -421,47 +389,32 @@ const __grid_constant__ TcArgs a) {
   const uint32_t emptyA = smem_u32(&bars[TC_MAX_STAGES]);
   const uint32_t fullB = smem_u32(&bars[2 * TC_MAX_STAGES]);
   const uint32_t emptyB = smem_u32(&bars[3 * TC_MAX_STAGES]);
-  const uint32_t tfull0 = smem_u32(&bars[4 * TC_MAX_STAGES]);
-  const uint32_t tempty0 = smem_u32(&bars[4 * TC_MAX_STAGES + TC_MAX_ACC]);
-  const uint32_t bfull = smem_u32(&bars[4 * TC_MAX_STAGES + 2 * TC_MAX_ACC]);
+  const uint32_t bfull = smem_u32(&bars[4 * TC_MAX_STAGES]);
 
   // PDL: let the next kernel of the stream/graph start its prologue while this grid runs; it blocks in
   // its own griddepcontrol.wait until this grid has completed and flushed.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (warp == 0 && lane == 0) {
+  if (warp == TC_CONSUMER_WARPS && lane == 0) {
     s_head = 0;
     for (int s = 0; s < a.stages_a; s++) {
       mbar_init(fullA + 8 * s, 1);
-      mbar_init(emptyA + 8 * s, 1);
+      mbar_init(emptyA + 8 * s, TC_CONSUMER_WARPS);
     }
     for (int s = 0; s < a.stages_b; s++) {
       mbar_init(fullB + 8 * s, 1);
-      mbar_init(emptyB + 8 * s, 1);
-    }
-    for (int s = 0; s < a.n_acc; s++) {
-      mbar_init(tfull0 + 8 * s, 1);
-      mbar_init(tempty0 + 8 * s, 4);  // one arrive per warp of the draining epilogue group
+      mbar_init(emptyB + 8 * s, TC_CONSUMER_WARPS);
     }
     mbar_init(bfull, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)),
-                 "r"(a.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
 
   const int taps = a.ksz * a.ksz;
   const int tiles_per_img = a.tiles_w * a.tiles_h;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == TC_CONSUMER_WARPS && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmA) : "memory");
     if (a.b_resident) {
       // weights do not depend on the previous kernel: fetch them before the grid dependency resolves
@@ -474,63 +427,15 @@ const __grid_constant__ TcArgs a) {
   // its producer by per-image counters (dep_ctr): then tiles start as soon as their images are complete
   if (a.dep_ctr == nullptr) asm volatile("griddepcontrol.wait;" ::: "memory");
 
-  if (warp == 0) {
+  const bool dyn = a.tile_ctr != nullptr;
+  if (warp == TC_CONSUMER_WARPS) {
     // ===================== TMA producer =====================
     if (lane == 0) {
-      if (a.dual) {
-        // pairs of tiles (same N tile: the grid is a multiple of n_tiles) share every weight slab
-        const int ra = a.stages_a, rb = a.stages_b;
-        int sa = 0, sb = 0;
-        uint32_t pa = 0, pb = 0;
-        for (int tile0 = blockIdx.x; tile0 < a.total_tiles; tile0 += 2 * gridDim.x) {
-          const int nT = (tile0 + (int)gridDim.x < a.total_tiles) ? 2 : 1;
-          int img_[2], wc_[2], hb_[2], nt = 0;
-          for (int q = 0; q < nT; q++) {
-            const int tile = tile0 + q * gridDim.x;
-            const int mt = fdiv(tile, a.m_ntiles);
-            nt = tile - mt * a.n_tiles;
-            img_[q] = fdiv(mt, a.m_tpi);
-            const int r = mt - img_[q] * tiles_per_img;
-            const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
-            wc_[q] = a.mode == TC_S2P ? tw * a.BW - 1 : tw * a.BW * a.stride - a.pad;
-            hb_[q] = th * a.BH * a.stride - a.pad;
-          }
-          auto load_a = [&](int q, int c0, int dw, int dh) {
-            mbar_wait(emptyA + 8 * sa, pa ^ 1);
-            mbar_arrive_expect_tx(fullA + 8 * sa, a.a_bytes);
-            tma_load_4d(smemA + sa * a.a_stride, &a.tmA, fullA + 8 * sa, c0, wc_[q] + dw, hb_[q] + dh, img_[q]);
-            if (++sa == ra) { sa = 0; pa ^= 1; }
-          };
-          auto load_b = [&](int t, int ch) {
-            mbar_wait(emptyB + 8 * sb, pb ^ 1);
-            mbar_arrive_expect_tx(fullB + 8 * sb, a.b_bytes);
-            bulk_load_1d(smemB + sb * a.b_stride, a.wpk + (size_t)((nt * taps + t) * a.chunks + ch) * a.b_stride, a.b_bytes,
-                         fullB + 8 * sb);
-            if (++sb == rb) { sb = 0; pb ^= 1; }
-          };
-          if (a.mode != TC_TAP) {
-            for (int ch = 0; ch < a.chunks; ch++) {
-              for (int q = 0; q < nT; q++) load_a(q, ch * a.BK, 0, 0);
-              for (int t = 0; t < taps; t++) load_b(t, ch);
-            }
-          } else {
-            for (int t = 0; t < taps; t++) {
-              const int kh = a.ksz == 3 ? (t >= 6 ? 2 : (t >= 3 ? 1 : 0)) : 0, kw = t - kh * a.ksz;
-              for (int ch = 0; ch < a.chunks; ch++) {
-                for (int q = 0; q < nT; q++) load_a(q, ch * a.BK, kw, kh);
-                load_b(t, ch);
-              }
-            }
-          }
-        }
-      }
-      const int ni = a.n_issuers;
-      const int ra = a.stages_a / ni, rb = a.b_resident ? 0 : a.stages_b / ni;
-      int sa_[2] = {0, 0}, sb_[2] = {0, 0};
-      uint32_t pa_[2] = {0, 0}, pb_[2] = {0, 0};
+      const int ra = a.stages_a, rb = a.b_resident ? 0 : a.stages_b;
+      int sa = 0, sb = 0;
+      uint32_t pa = 0, pb = 0;
       int li = 0;
-      const bool dyn = a.tile_ctr != nullptr;
-      int tile = a.dual ? a.total_tiles : (int)blockIdx.x;
+      int tile = (int)blockIdx.x;
       int nxt = a.total_tiles, left = 1;
       const int batch = a.tile_batch;
       // the next batch of tiles is drawn one batch ahead, so the atomic's latency never sits on the load path
@@ -555,10 +460,6 @@ const __grid_constant__ TcArgs a) {
           }
         }
         if (dyn) tq_publish(s_tile, &s_head, li, tile);
-        const int rg = ni == 2 ? (li & 1) : 0;  // ring (= issuer) of this tile
-        int& sa = sa_[rg]; int& sb = sb_[rg];
-        uint32_t& pa = pa_[rg]; uint32_t& pb = pb_[rg];
-        const int a_base = rg * ra, b_base = rg * rb;
         const int mt = fdiv(tile, a.m_ntiles);
         const int nt = tile - mt * a.n_tiles;
         const int img = fdiv(mt, a.m_tpi);
@@ -566,40 +467,32 @@ const __grid_constant__ TcArgs a) {
         const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
         const int wbase = tw * a.BW * a.stride - a.pad;
         const int hbase = th * a.BH * a.stride - a.pad;
+        auto load_b = [&](int t, int ch) {
+          mbar_wait(emptyB + 8 * sb, pb ^ 1);
+          mbar_arrive_expect_tx(fullB + 8 * sb, a.b_bytes);
+          bulk_load_1d(smemB + sb * a.b_stride, a.wpk + (size_t)((nt * taps + t) * a.chunks + ch) * a.b_stride, a.b_bytes,
+                       fullB + 8 * sb);
+          if (++sb == rb) { sb = 0; pb ^= 1; }
+        };
         if (a.mode != TC_TAP) {
           for (int ch = 0; ch < a.chunks; ch++) {
-            mbar_wait(emptyA + 8 * (a_base + sa), pa ^ 1);
-            mbar_arrive_expect_tx(fullA + 8 * (a_base + sa), a.a_bytes);
-            tma_load_4d(smemA + (a_base + sa) * a.a_stride, &a.tmA, fullA + 8 * (a_base + sa), ch * a.BK,
-                        a.mode == TC_S2P ? tw * a.BW - 1 : wbase, hbase, img);
+            mbar_wait(emptyA + 8 * sa, pa ^ 1);
+            mbar_arrive_expect_tx(fullA + 8 * sa, a.a_bytes);
+            tma_load_4d(smemA + sa * a.a_stride, &a.tmA, fullA + 8 * sa, ch * a.BK, a.mode == TC_S2P ? tw * a.BW - 1 : wbase,
+                        hbase, img);
             if (++sa == ra) { sa = 0; pa ^= 1; }
             if (!a.b_resident)
-              for (int t = 0; t < taps; t++) {
-                mbar_wait(emptyB + 8 * (b_base + sb), pb ^ 1);
-                mbar_arrive_expect_tx(fullB + 8 * (b_base + sb), a.b_bytes);
-                bulk_load_1d(smemB + (b_base + sb) * a.b_stride,
-                             a.wpk + (size_t)((nt * taps + t) * a.chunks + ch) * a.b_stride, a.b_bytes,
-                             fullB + 8 * (b_base + sb));
-                if (++sb == rb) { sb = 0; pb ^= 1; }
-              }
+              for (int t = 0; t < taps; t++) load_b(t, ch);
           }
         } else {
           for (int t = 0; t < taps; t++) {
             const int kh = a.ksz == 3 ? (t >= 6 ? 2 : (t >= 3 ? 1 : 0)) : 0, kw = t - kh * a.ksz;
             for (int ch = 0; ch < a.chunks; ch++) {
-              mbar_wait(emptyA + 8 * (a_base + sa), pa ^ 1);
-              mbar_arrive_expect_tx(fullA + 8 * (a_base + sa), a.a_bytes);
-              tma_load_4d(smemA + (a_base + sa) * a.a_stride, &a.tmA, fullA + 8 * (a_base + sa), ch * a.BK, wbase + kw,
-                          hbase + kh, img);
+              mbar_wait(emptyA + 8 * sa, pa ^ 1);
+              mbar_arrive_expect_tx(fullA + 8 * sa, a.a_bytes);
+              tma_load_4d(smemA + sa * a.a_stride, &a.tmA, fullA + 8 * sa, ch * a.BK, wbase + kw, hbase + kh, img);
               if (++sa == ra) { sa = 0; pa ^= 1; }
-              if (!a.b_resident) {
-                mbar_wait(emptyB + 8 * (b_base + sb), pb ^ 1);
-                mbar_arrive_expect_tx(fullB + 8 * (b_base + sb), a.b_bytes);
-                bulk_load_1d(smemB + (b_base + sb) * a.b_stride,
-                             a.wpk + (size_t)((nt * taps + t) * a.chunks + ch) * a.b_stride, a.b_bytes,
-                             fullB + 8 * (b_base + sb));
-                if (++sb == rb) { sb = 0; pb ^= 1; }
-              }
+              if (!a.b_resident) load_b(t, ch);
             }
           }
         }
@@ -615,192 +508,42 @@ const __grid_constant__ TcArgs a) {
           tile += gridDim.x;
         }
       }
-      if (dyn && !a.dual) {  // end marks for every reader (2 issuers, up to 4 epilogue groups)
-        for (int k = 0; k < 3; k++) s_tile[(li + k) & (TQ - 1)] = -1;
-        tq_publish(s_tile, &s_head, li + 3, -1);
-      }
-    }
-  } else if (warp == 1 || warp == 2) {
-    // ===================== MMA issuers (whole warp, elect.sync issues) =====================
-    {
-      const int issuer = warp - 1;
-      if (a.dual) {
-        if (issuer == 0) {
-          switch (a.BK) {
-            case 64: mma_role_dual<4>(a, smemA, smemB, tmem_base, fullA, emptyA, fullB, emptyB, tfull0, tempty0); break;
-            case 32: mma_role_dual<2>(a, smemA, smemB, tmem_base, fullA, emptyA, fullB, emptyB, tfull0, tempty0); break;
-            default: mma_role_dual<1>(a, smemA, smemB, tmem_base, fullA, emptyA, fullB, emptyB, tfull0, tempty0); break;
-          }
-        }
-      } else
-      switch (a.BK) {
-        case 64: mma_role<4>(a, smemA, smemB, tmem_base, fullA, emptyA, fullB, emptyB, tfull0, tempty0, bfull, issuer, s_tile, &s_head); break;
-        case 32: mma_role<2>(a, smemA, smemB, tmem_base, fullA, emptyA, fullB, emptyB, tfull0, tempty0, bfull, issuer, s_tile, &s_head); break;
-        default: mma_role<1>(a, smemA, smemB, tmem_base, fullA, emptyA, fullB, emptyB, tfull0, tempty0, bfull, issuer, s_tile, &s_head); break;
-      }
+      if (dyn) tq_publish(s_tile, &s_head, li, -1);  // end mark
     }
   } else {
-    // ===================== epilogue (warps 3 ..) =====================
-    // G groups of four warps (one warp per TMEM lane quarter: a warp may only read lanes
-    // 32*(warp%4)..+31; any four consecutive warps cover all quarters) drain different tiles: group g
-    // takes local tiles g, g+G, ...  The per-tile epilogue is a latency-bound ~2000-4000 cycle chain
-    // (tcgen05.ld -> bias -> SiLU -> pack -> store), so its THROUGHPUT comes from having several tiles in
-    // their epilogue at once (timeline: one tile at a time paced the whole kernel for N <= 64).
-    const int ew = warp - 3;
-    const int q = warp & 3;
-    const int grp = ew >> 2;
-    const int G = a.n_groups;
-    const int row = q * 32 + lane;
-    const bool dyn = a.tile_ctr != nullptr;
+    // ===================== consumers: wgmma main loop + epilogue =====================
+    const int wg = warp >> 2;
+    int sa = 0, sb = 0;
+    uint32_t pa = 0, pb = 0;
+    if (a.b_resident) mbar_wait(bfull, 0);
     int pend_img = -1, pend_cnt = 0;  // layer chaining: rows stored but not yet published
-    for (int li = grp;; li += G) {
+    const bool dbg_on = a.dbg && blockIdx.x == 0 && threadIdx.x == 0;
+    for (int li = 0;; li++) {
       const int tile = dyn ? tq_get(s_tile, &s_head, li) : (int)blockIdx.x + li * (int)gridDim.x;
       if (tile < 0 || tile >= a.total_tiles) break;
-      const int acc = li & (a.n_acc - 1);  // n_acc is 2 or 4
-      const uint32_t aphase = (uint32_t)(li >> (a.n_acc == 4 ? 2 : 1)) & 1u;
+      if (dbg_on && li < 16) a.dbg[li * 8 + 0] = clock64();
+      float acc[NT16 * 8];
+      switch (a.BK) {
+        case 64: tc_mainloop<NT16, 4>(a, acc, wg, smemA, smemB, fullA, emptyA, fullB, emptyB, sa, pa, sb, pb); break;
+        case 32: tc_mainloop<NT16, 2>(a, acc, wg, smemA, smemB, fullA, emptyA, fullB, emptyB, sa, pa, sb, pb); break;
+        default: tc_mainloop<NT16, 1>(a, acc, wg, smemA, smemB, fullA, emptyA, fullB, emptyB, sa, pa, sb, pb); break;
+      }
+      if (dbg_on && li < 16) a.dbg[li * 8 + 3] = clock64();
       const int mt = fdiv(tile, a.m_ntiles);
       const int nt = tile - mt * a.n_tiles;
       const int img = fdiv(mt, a.m_tpi);
       const int r = mt - img * tiles_per_img;
       const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
-      const int hl = fdiv(row, a.m_bw), wl = row - hl * a.BW;
-      const int ho = th * a.BH + hl, wo = tw * a.BW + wl;
-      const bool valid = hl < a.BH && ho < a.Ho && wo < a.Wo;
-      const size_t pix = ((size_t)img * a.Ho + ho) * a.Wo + wo;
       const int n0 = nt * a.n_tile;
-      const float* bias = s_bias + n0;
-      int4 rv[4];
-      const bool use_res = a.epi_mode == EPI_STORE && a.res != nullptr;
-      if (use_res) res_prefetch(a, n0, 0, pix, valid, rv);
-
-      const int dbg_t = li;
-      const bool dbg_on = a.dbg && blockIdx.x == 0 && (warp & 3) == 3 && lane == 0 && dbg_t < 16;
-      if (dbg_on) a.dbg[dbg_t * 8 + 4] = clock64();
-      mbar_wait(tfull0 + 8 * acc, aphase);
-      tc_fence_after();
-      if (dbg_on) a.dbg[dbg_t * 8 + 5] = clock64();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * a.n_tile;
-      if (a.epi_mode != EPI_STORE) {
-        // fused Detect tail (flattened 1x1 conv): this thread's row is pixel `wo` of the whole batch
-        const int n = valid ? wo / a.dHW : 0;
-        const int i = wo - n * a.dHW;
-        float* po = a.pred + (size_t)n * a.dCtot * a.dA + a.da0 + i;
-        if (a.epi_mode == EPI_DFL_BOX) {
-          // DFL (Block.cs:44): softmax over the 16 bins of each side, expectation with weights 0..15;
-          // then dist2bbox(xywh) * stride (Tal.cs:338-356, Head.cs:221)
-          float d[4];
-#pragma unroll
-          for (int sd = 0; sd < 4; sd++) {
-            uint32_t v[16];
-            tmem_ld16(taddr + sd * 16, v);
-            tmem_ld_wait();
-            float f[16], mx = -INFINITY;
-#pragma unroll
-            for (int j = 0; j < 16; j++) { f[j] = __uint_as_float(v[j]) + bias[sd * 16 + j]; mx = fmaxf(mx, f[j]); }
-            float sum = 0.f, ex = 0.f;
-#pragma unroll
-            for (int j = 0; j < 16; j++) { const float e = __expf(f[j] - mx); sum += e; ex = fmaf(e, (float)j, ex); }
-            d[sd] = __fdividef(ex, sum);
-          }
-          if (valid) {
-            const int y = i / a.dWl, x = i - y * a.dWl;
-            const float ax = (float)x + 0.5f, ay = (float)y + 0.5f;
-            const float x1 = ax - d[0], y1 = ay - d[1], x2 = ax + d[2], y2 = ay + d[3];
-            po[0] = (x1 + x2) * 0.5f * a.dstride;
-            po[(size_t)a.dA] = (y1 + y2) * 0.5f * a.dstride;
-            po[(size_t)2 * a.dA] = (x2 - x1) * a.dstride;
-            po[(size_t)3 * a.dA] = (y2 - y1) * a.dstride;
-          }
-        } else {
-          for (int c0 = 0; c0 < a.n_tile; c0 += 16) {
-            uint32_t v[16];
-            tmem_ld16(taddr + c0, v);
-            tmem_ld_wait();
-            if (valid) {
-#pragma unroll
-              for (int j = 0; j < 16; j++) {
-                float f = __uint_as_float(v[j]) + bias[c0 + j];
-                if (a.epi_mode == EPI_SIGMOID) f = __fdividef(1.0f, 1.0f + __expf(-f));
-                po[(size_t)(a.dch0 + c0 + j) * a.dA] = f;  // lanes = consecutive anchors: coalesced
-              }
-            }
-          }
-        }
-      } else {
-        // Store path, 32 columns at a time.  A lane owns one output pixel (TMEM lane) and writes its own
-        // 64 contiguous bytes per block with four 16-byte stores.
-        // (A smem-transposed variant that made every warp store cover whole rows cut L2 requests 8x but
-        // cost ~1000 cycles of shuffles / smem round trips per tile; ncu shows L2 far from saturated,
-        // so the short instruction path wins.)
-        __half* orow = a.out + pix * a.out_pitch + a.out_coff + n0;
-        for (int cb0 = 0; cb0 < a.n_tile; cb0 += 32) {
-          const int wb = min(32, a.n_tile - cb0);  // 32 or 16 channels
-          uint32_t v[32];
-          if (wb == 32) tmem_ld32(taddr + cb0, v); else tmem_ld16(taddr + cb0, *reinterpret_cast<uint32_t(*)[16]>(&v[0]));
-          tmem_ld_wait();
-#pragma unroll
-          for (int g = 0; g < 4; g++) {  // 8 channels -> one 16-byte store
-            if (g * 8 < wb) {
-              const float4 b0 = *reinterpret_cast<const float4*>(bias + cb0 + g * 8);
-              const float4 b1 = *reinterpret_cast<const float4*>(bias + cb0 + g * 8 + 4);
-              float f[8];
-              f[0] = __uint_as_float(v[g * 8 + 0]) + b0.x; f[1] = __uint_as_float(v[g * 8 + 1]) + b0.y;
-              f[2] = __uint_as_float(v[g * 8 + 2]) + b0.z; f[3] = __uint_as_float(v[g * 8 + 3]) + b0.w;
-              f[4] = __uint_as_float(v[g * 8 + 4]) + b1.x; f[5] = __uint_as_float(v[g * 8 + 5]) + b1.y;
-              f[6] = __uint_as_float(v[g * 8 + 6]) + b1.z; f[7] = __uint_as_float(v[g * 8 + 7]) + b1.w;
-              if (a.act == ACT_SILU) {
-#pragma unroll
-                for (int j = 0; j < 8; j++) f[j] = silu_tanh(f[j]);
-              }
-              if (use_res) {
-                const __half2* h = reinterpret_cast<const __half2*>(&rv[g]);
-#pragma unroll
-                for (int j = 0; j < 4; j++) {
-                  const float2 x = __half22float2(h[j]);
-                  f[2 * j] += x.x; f[2 * j + 1] += x.y;
-                }
-              }
-              int4 o;
-              __half2* ph = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-              for (int j = 0; j < 4; j++) ph[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-              if (valid) *reinterpret_cast<int4*>(orow + cb0 + g * 8) = o;
-            }
-          }
-          if (use_res && cb0 + 32 < a.n_tile) res_prefetch(a, n0, cb0 + 32, pix, valid, rv);  // next block
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
+      bool valid[2];
+      int wo[2];
+      tc_epilogue<NT16>(a, acc, s_bias + n0, n0, img, th, tw, wg, valid, wo);
       if (a.done_ctr != nullptr && a.epi_mode == EPI_STORE) {
-        // Publish this warp's rows per image.  A publish is fence (every lane's stores before the count) + warp barrier
-        // + one atomic; the fence costs several hundred cycles on the epilogue's latency chain, so rows are counted in
-        // registers and published only when the warp moves on to another image (tiles arrive in image order) or runs
-        // out of tiles.  A flattened tile may span two images.
-        const int my_img = (a.imgs == 1 && a.Ho == 1) ? fdiv(min(wo, a.Wo - 1), a.m_ohw) : img;
-        const unsigned vm = __ballot_sync(0xffffffffu, valid);
-        if (vm) {
-          const int first = __shfl_sync(0xffffffffu, my_img, __ffs(vm) - 1);
-          const unsigned same = __ballot_sync(0xffffffffu, valid && my_img == first);
-          if (pend_img >= 0 && pend_img != first) {
-            __threadfence();
-            __syncwarp();
-            if (lane == 0) atomicAdd(a.done_ctr + pend_img, pend_cnt);
-            pend_cnt = 0;
-          }
-          pend_img = first;
-          pend_cnt += __popc(same);
-          if (vm != same) {
-            __threadfence();
-            __syncwarp();
-            if (lane == 0) atomicAdd(a.done_ctr + first, pend_cnt);
-            pend_img = first + 1;
-            pend_cnt = __popc(vm ^ same);
-          }
-        }
+        const bool flat1 = a.imgs == 1 && a.Ho == 1;
+        const int im[2] = {flat1 ? fdiv(min(wo[0], a.Wo - 1), a.m_ohw) : img, flat1 ? fdiv(min(wo[1], a.Wo - 1), a.m_ohw) : img};
+        chain_count(a, valid, im, pend_img, pend_cnt);
       }
-      if (dbg_on) a.dbg[dbg_t * 8 + 6] = clock64();
+      if (dbg_on && li < 16) a.dbg[li * 8 + 6] = clock64();
     }
     if (pend_img >= 0) {
       __threadfence();
@@ -808,18 +551,11 @@ const __grid_constant__ TcArgs a) {
       if (lane == 0) atomicAdd(a.done_ctr + pend_img, pend_cnt);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(a.tmem_cols) : "memory");
-  }
 }
 
 // One-time weight packing: w [Cout][tap][Cin] fp16 -> slab images [n tile][tap][chunk][b_stride bytes]; inside a
 // slab row r (output channel) holds BK channels, its 16-byte piece c sits at the K-major swizzled position the
-// UMMA descriptor expects: c ^ (r & 7) for 128-byte rows, c ^ ((r >> 1) & 3) for 64-byte, c ^ ((r >> 2) & 1) for 32-byte.
+// wgmma descriptor expects: c ^ (r & 7) for 128-byte rows, c ^ ((r >> 1) & 3) for 64-byte, c ^ ((r >> 2) & 1) for 32-byte.
 __global__ void pack_weights_kernel(const __half* __restrict__ w, uint8_t* __restrict__ out, int n_tile, int n_tiles,
                                     int taps, int chunks, int BK, int Cin, uint32_t b_stride, long long pieces) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -865,8 +601,7 @@ bool tc_conv_supported(const ConvParams& p) {
   return true;
 }
 
-// Experiment knob (tools/exp_dual.py): YB_PLAN_SMALL=1 sizes every plan for half an SM (<= 104 KiB of rings, <= 256
-// TMEM columns, 352 threads) and launches one CTA per SM, so that kernels of TWO concurrent streams (two half-batch
+// Experiment knob (tools/exp_dual.py): YB_PLAN_SMALL=1 sizes every plan for half an SM (<= 104 KiB of rings) and launches one CTA per SM, so that kernels of TWO concurrent streams (two half-batch
 // engines) are co-resident on every SM and each fills the other's pipeline bubbles.
 static int plan_small() {
   const char* v = getenv("YB_PLAN_SMALL");
@@ -901,9 +636,8 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
   a.mode = (p.k == 3 && p.stride == 1) ? TC_HALO : (s2p_ok ? TC_S2P : TC_TAP);
   // channel slab: the widest of 64 / 32 / 16 channels (128 / 64 / 32-byte operand rows) that pads K by at most
   // 35 %; a ragged last slab
-  // is zero-filled by TMA (activations, dim 0 bound = Cin) and by the weight packing.  (80 / 160 / 400-channel
-  // layers of v8x ran with 16 / 32-channel slabs = 32 / 64-byte rows and stayed at ~30 % of the tensor peak while
-  // the 320 / 640-channel layers reached 45-75 %.)
+  // is zero-filled by TMA (activations, dim 0 bound = Cin) and by the weight packing.  (Wider rows mean fewer, longer
+  // MMA K steps per slab.)
   auto padded = [&](int bk) { return (p.Cin + bk - 1) / bk * bk; };
   a.BK = padded(64) * 100 <= p.Cin * 135 ? 64 : (padded(32) * 100 <= p.Cin * 135 ? 32 : 16);  // <= 35 % zero K
   a.chunks = (p.Cin + a.BK - 1) / a.BK;
@@ -912,19 +646,18 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
   a.n_tiles = p.Cout / a.n_tile;
   const CUtensorMapSwizzle swz = a.BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
                                             : (a.BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-  a.layout_a = a.layout_b = a.BK == 64 ? 2 : (a.BK == 32 ? 4 : 6);
+  a.layout_a = a.layout_b = a.BK == 64 ? 1 : (a.BK == 32 ? 2 : 3);
   a.row_bytes = a.BK * 2;
   a.sbo_a = a.sbo_b = (8 * a.row_bytes) >> 4;
   // stride-2 3x3, pair rows: two horizontally adjacent pixels (input columns 2q, 2q+1) are contiguous in a
   // whole-buffer NHWC view, so the tensor map declares them as ONE row of 2*Cin channels with the swizzle of
   // that width.  One dense box of (2BH+1) input rows x (BW+1) pairs then serves all 9 taps as row / K-slice
-  // shifts (see mma_role); the left / top zero padding is TMA out-of-bounds fill of pair -1 / row -1.
-  // (A strided box per tap moved 9 x 128 rows of Cin*2 bytes per tile and was bound by the TMA row rate:
-  //  93 G sectors/s on model.1, profiles/r1_ncu_s2_tap_mode.txt.)
+  // shifts (see tc_mainloop); the left / top zero padding is TMA out-of-bounds fill of pair -1 / row -1.
+  // (A strided box per tap moves 9 x 128 rows of Cin*2 bytes per tile and is bound by the TMA row rate.)
   CUtensorMapSwizzle swz_a = swz;
   if (a.mode == TC_S2P) {
     swz_a = a.BK == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    a.layout_a = a.BK == 32 ? 2 : 4;
+    a.layout_a = a.BK == 32 ? 1 : 2;
   }
 
   plan->flat = (p.k == 1 && p.stride == 1);
@@ -992,8 +725,7 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
   {
     // Weights are constant: store every [n_tile x BK] slab in global memory exactly as it must look in shared
     // memory (swizzled rows, padded to b_stride), so the kernel fetches a slab with ONE contiguous bulk copy.
-    // (As 2-D TMA boxes the slabs cost ~3 cycles per row in the TMA unit - 7200 rows per tile for a 3x3 160->160
-    //  layer, more than its MMAs - and bounded the wide layers of v8s / v8x at ~30 % of the tensor peak.)
+    // (As 2-D TMA boxes the slabs would cost the TMA unit one row each - 7200 rows per tile for a 3x3 160->160 layer.)
     const size_t total = (size_t)a.n_tiles * a.ksteps * a.b_stride;
     if (cudaMalloc(&plan->wpk, total) != cudaSuccess) {
       if (err) *err = "cudaMalloc(packed weights) failed";
@@ -1015,14 +747,16 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
     }
     a.wpk = plan->wpk;
   }
-  // Two CTAs per SM (each <= ~100 KiB smem, <= 256 TMEM columns) double the tiles in flight per SM and
-  // hide the producer -> MMA -> epilogue hand-off latencies of the HBM-bound high-resolution layers;
-  // layers whose resident weights or wide N tiles do not fit run one CTA per SM with the full budget.
-  // 4 accumulator buffers when they fit in 256 TMEM columns (keeps two CTAs per SM possible), else 2
-  a.n_acc = 4 * a.n_tile <= 256 ? 4 : 2;
-  uint32_t cols = 32;
-  while (cols < (uint32_t)(a.n_acc * a.n_tile)) cols <<= 1;
-  a.tmem_cols = cols;
+  // Two CTAs per SM (each <= ~100 KiB smem) double the tiles in flight per SM and hide the producer -> MMA ->
+  // epilogue hand-off latencies of the HBM-bound high-resolution layers; they need n_tile <= 64 (the register budget of
+  // two 288-thread CTAs leaves room for 32 accumulator registers per thread).  Layers whose resident weights or wide N
+  // tiles do not fit run one CTA per SM with the full budget.
+  static int num_sms = 0;
+  if (!num_sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+  }
   const size_t b_all = (size_t)a.ksteps * a.b_stride;
   const int m_tiles = plan->flat ? (p.B * p.Ho * p.Wo + 127) / 128
                                  : p.B * ((p.Wo + a.BW - 1) / a.BW) * ((p.Ho + a.BH - 1) / a.BH);
@@ -1031,8 +765,8 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
     const size_t budget = occ == 2 ? 104 * 1024 : 200 * 1024;  // operand rings
     // layers with <= 2 tiles per CTA gain nothing from deep rings or resident weights; a small footprint
     // lets the NEXT kernel's CTAs (PDL / sibling branches) become resident while this one drains
-    const bool small = m_tiles * a.n_tiles <= 2 * 148;
-    if (occ == 2 && cols > 256) continue;
+    const bool small = m_tiles * a.n_tiles <= 2 * num_sms;
+    if (occ == 2 && a.n_tile > 64) continue;
     // keep the whole weight matrix in smem when it leaves room for >= 3 activation slabs: removes the
     // weight re-fetch per tile
     a.b_resident = (a.n_tiles == 1 && b_all + 3 * (size_t)a.a_stride <= budget) ? 1 : 0;
@@ -1057,43 +791,6 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
     if (fits && (occ == 1 || small || a.stages_a >= 3 || plan_small())) { plan->occ = occ; break; }
     if (occ == 1) a.stages_a = 0;  // reported below
   }
-  // epilogue groups: one per accumulator buffer at one CTA/SM (608 threads); two when two CTAs share the SM
-  a.n_groups = (plan->occ == 1 && a.n_acc == 4) ? 4 : 2;
-  plan->threads = 96 + 128 * a.n_groups;
-  // two issuers need >= 2 slabs per half ring
-  a.n_issuers = (a.stages_a >= 4 && (a.b_resident || a.stages_b >= 4)) ? 2 : 1;
-  {
-    // Each issuer owns half of the ring and the single producer fills tiles in order: when a half ring cannot hold
-    // one tile's activation slabs plus one of the next tile, the producer blocks inside a tile and the other
-    // issuer starves (timeline of the 3-slab 80->80 layers of v8x: the two issuers alternated instead of
-    // overlapping).  Such layers run one issuer on the whole ring.
-    const int slabs_per_tile = a.mode != TC_TAP ? a.chunks : a.ksteps;
-    if (a.n_issuers == 2 && a.stages_a / 2 < slabs_per_tile + 1) a.n_issuers = 1;
-  }
-  if (a.n_issuers == 2) {
-    a.stages_a &= ~1;  // even split
-    if (!a.b_resident) a.stages_b &= ~1;
-  }
-  if (!a.b_resident) {
-    // streamed weights: tile pairs share the weight slabs (mma_role_dual); two activation slabs per step
-    const size_t budget = plan->occ == 2 ? 104 * 1024 : 200 * 1024;
-    int sa2, sb2;
-    if (a.mode != TC_TAP) {
-      sa2 = (size_t)4 * a.a_stride + 3 * (size_t)a.b_stride <= budget ? 4 : 2;
-      sb2 = budget > (size_t)sa2 * a.a_stride ? (int)std::min<size_t>(TC_MAX_STAGES, (budget - (size_t)sa2 * a.a_stride) / a.b_stride) : 0;
-    } else {
-      const int S = (int)std::min<size_t>(6, budget / (2 * (size_t)a.a_stride + a.b_stride));
-      sa2 = 2 * S;
-      sb2 = S;
-    }
-    if (sa2 >= 2 && sb2 >= 2) {
-      a.dual = 1;
-      a.n_issuers = 1;
-      a.stages_a = sa2;
-      a.stages_b = sb2;
-      plan->smem = (size_t)a.stages_a * a.a_stride + (size_t)a.stages_b * a.b_stride + 1024;
-    }
-  }
   if (a.stages_a < 2 || (!a.b_resident && a.stages_b < 2)) {
     if (err) *err = "tile does not fit in shared memory";
     delete plan;
@@ -1107,33 +804,29 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
     delete plan;
     return nullptr;
   }
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+  dispatch_nt16(a.n_tile / 16, [&](auto nt16) { plan->kernel = conv_tc_kernel<decltype(nt16)::value>; });
+  {
     // dynamic limit = ring budget + alignment slack (static smem of the kernel counts against the 227 KiB cap)
-    cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaError_t ce = cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 202 * 1024);
+    cudaFuncSetAttribute(plan->kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaError_t ce = cudaFuncSetAttribute(plan->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 202 * 1024);
     if (ce != cudaSuccess) {
       if (err) *err = std::string("cudaFuncSetAttribute(conv_tc_kernel) failed: ") + cudaGetErrorString(ce);
-      num_sms = 0;
       delete plan;
       return nullptr;
     }
   }
   plan->grid = num_sms * plan->occ;
   if (plan_small() && plan->occ == 2) plan->grid = num_sms;  // the SM's other half belongs to the other stream's kernel
-  plan->small = m_tiles * a.n_tiles <= 2 * 148;
+  plan->small = m_tiles * a.n_tiles <= 2 * num_sms;
   return plan;
 }
 
 std::string tc_conv_plan_describe(const TcConvPlan* plan) {
   const TcArgs& a = plan->args;
   char buf[256];
-  snprintf(buf, sizeof(buf), "mode %d BK %d chunks %d n_tile %d x%d stages a/b %d/%d resident %d dual %d issuers %d groups %d acc %d occ %d "
-           "threads %d smem %zu KiB grid %d", a.mode, a.BK, a.chunks, a.n_tile, a.n_tiles, a.stages_a, a.stages_b, a.b_resident, a.dual,
-           a.n_issuers, a.n_groups, a.n_acc, plan->occ, plan->threads, plan->smem / 1024, plan->grid);
+  snprintf(buf, sizeof(buf), "mode %d BK %d chunks %d n_tile %d x%d stages a/b %d/%d resident %d occ %d threads %d smem %zu KiB grid %d",
+           a.mode, a.BK, a.chunks, a.n_tile, a.n_tiles, a.stages_a, a.stages_b, a.b_resident, plan->occ, TC_THREADS, plan->smem / 1024,
+           plan->grid);
   return buf;
 }
 
@@ -1142,7 +835,7 @@ void tc_conv_plan_destroy(TcConvPlan* plan) {
   delete plan;
 }
 
-long long* g_tc_dbg = nullptr;  // set by yb_debug_timeline: next tcgen05 conv launches write their timeline here
+long long* g_tc_dbg = nullptr;  // set by yb_debug_timeline: next tensor-core conv launches write their timeline here
 int g_tc_dbg_countdown = -1;
 
 int tc_conv_rows_per_image(const TcConvPlan* plan) { return plan->p.Ho * plan->p.Wo * plan->args.n_tiles; }
@@ -1152,14 +845,10 @@ int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cu
   a.pred = pred;
   if (chain) {
     a.done_ctr = chain->done_ctr;
-    if (!plan->args.dual) {  // tile pairs (streamed weights, static order) keep the grid-wide dependency
-      a.dep_ctr = chain->dep_ctr;
-      a.dep_expect = chain->dep_expect;
-    }
+    a.dep_ctr = chain->dep_ctr;
+    a.dep_expect = chain->dep_expect;
   }
-  // Tile pairs keep the static order (both tiles need the same N tile).  (Restricting the queue to long-tile layers
-  // made the isolated short-tile layers of v8n ~10 % faster but the overlapped step no faster, and cost v8s 4 %.)
-  a.tile_ctr = a.dual ? nullptr : tile_ctr;
+  a.tile_ctr = tile_ctr;
   a.dbg = nullptr;
   if (g_tc_dbg && g_tc_dbg_countdown >= 0 && g_tc_dbg_countdown-- == 0) a.dbg = g_tc_dbg;
   const ConvParams& p = plan->p;
@@ -1183,18 +872,17 @@ int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cu
   // chained layers: one CTA per SM for the two-CTA plans, so that the other slot of every SM is free for the NEXT
   // layer's CTA - consecutive layers then run side by side, the later one on the images the earlier one has finished
   static const int chain_grid1 = getenv("YB_CHAIN_GRID1") ? atoi(getenv("YB_CHAIN_GRID1")) : 1;
-  if (chain && chain_grid1 && plan->occ == 2 && !a.dual) grid = std::min(grid, std::max(1, plan->grid / 2));
+  if (chain && chain_grid1 && plan->occ == 2) grid = std::min(grid, std::max(1, plan->grid / 2));
   // concurrent head branches: a latency-bound layer with ~1 tile per CTA gives up half of its CTAs (each
   // then pipelines 2-3 tiles) so that a sibling branch can occupy the other SMs at the same time
   if (plan->p.share_sms && a.total_tiles <= 4 * plan->grid && a.ksteps * (a.BK >> 4) <= 40)
     grid = std::max(1, std::min(grid, (a.total_tiles + 2) / 3));
-  if (a.dual && grid >= a.n_tiles) grid -= grid % a.n_tiles;  // tile t and t + grid must share their N tile
-  // one atomic per ~quarter of a CTA's share (every atomic of the grid hits the same L2 address: per-tile draws
-  // cost the 6400-tile layers 6-8 us)
+  // one atomic per ~quarter of a CTA's share (every atomic of the grid hits the same L2 address, so per-tile draws
+  // would serialise the 6400-tile layers)
   a.tile_batch = std::max(1, std::min(8, a.total_tiles / (4 * grid)));
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(plan->threads);
+  cfg.blockDim = dim3(TC_THREADS);
   cfg.dynamicSmemBytes = plan->smem;
   cfg.stream = s;
   cudaLaunchAttribute attr[1];
@@ -1203,7 +891,7 @@ int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cu
   cfg.attrs = attr;
   static const bool no_pdl = getenv("YB_DEBUG_NO_PDL") != nullptr;  // experiments only (tools/exp_fixed_cost.py)
   cfg.numAttrs = no_pdl ? 0 : 1;
-  YB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_tc_kernel, a));
+  YB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, plan->kernel, a));
   return 0;
 }
 
@@ -1213,19 +901,17 @@ int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cu
 // of the 9 (kh, c) input rows, the FOUR contiguous input columns 2wo-2 .. 2wo+1 form one 8-byte K group
 //     k = (kh*3 + c)*4 + slot,   slot 0 -> column 2wo-2 (weight 0), slots 1..3 -> kw = 0..2
 // so a thread builds its A row from 9 aligned 8-byte loads (K = 36, padded to 48 = 3 MMAs) instead of 27
-// scalar loads + repacking (the first version spent 650 instructions per warp and tile on that and was
-// issue-bound at 147 us; profiles/r1_ncu_stem_*.txt).
+// scalar loads + repacking.
 //   A tile   128 rows x 128 B, SWIZZLE_128B layout written by hand (16-byte piece p of row r at p ^ (r & 7))
 //   weights  [Cout][64] fp16 resident in smem, same layout
-//   MMA      3 x tcgen05.mma (M=128, N=Cout, K=16) by warp 4
-//   epilogue same 128 threads: tcgen05.ld -> +bias -> SiLU -> fp16 NHWC store (Cout*2 contiguous bytes)
+//   MMA      the same warpgroup: wgmma m64nNk16 for rows 0-63 and 64-127, K = 3 x 16, N = 64 output channels
+//            per pass (fewer in the last pass), fp32 accumulators in registers
+//   epilogue same 128 threads: +bias -> SiLU -> fp16 NHWC stores
 // Four CTAs per SM overlap each other's load / MMA / store latencies; the layer is HBM-bound
 // (reads the image once, writes Cout x H/2 x W/2 fp16).
-// (A TMA box load of the NCHW patch faulted with "illegal instruction" on B200 for rank-3 f32 maps;
-//  plain loads are used instead.)
 // ------------------------------------------------------------------------------------------
 constexpr int ST_TW = 16, ST_TH = 8;
-constexpr int ST_THREADS = 160;  // warps 0-3: im2col + epilogue, warp 4: MMA issue
+constexpr int ST_THREADS = 128;  // one warpgroup: im2col, MMA and epilogue
 
 struct StemArgs {
   const void* in;
@@ -1240,7 +926,6 @@ struct StemArgs {
   int src_H, src_W;
   uint32_t pad_h2;
   int tiles_w, tiles_h, total_tiles;
-  uint32_t tmem_cols;
   uint64_t m_tpi, m_tw;  // magic numbers for / tiles_per_img and / tiles_w (fdiv)
 };
 
@@ -1307,29 +992,51 @@ __device__ __forceinline__ uint2 stem_load4_ragged(const void* in, size_t rowbas
   return make_uint2(e[0] | (e[1] << 16), e[2] | (e[3] << 16));
 }
 
+// One pass of W (64 / 48 / 32 / 16) output channels c0.. of the current tile: 2 x 3 wgmma, then the epilogue of those
+// channels.  Row r of the tile is output pixel (tx, ty) = (r % 16, r / 16).
+template <int W>
+__device__ __forceinline__ void stem_pass(const StemArgs& a, uint32_t smA, uint32_t smB, const float* s_bias, int c0, int n,
+                                          int th, int tw) {
+  float acc[2][W / 2];
+  const uint32_t hi = wg_desc_hi(64, 1);  // SBO = 8 rows x 128 B, SWIZZLE_128B
+  wg_fence();
+#pragma unroll
+  for (int h = 0; h < 2; h++)
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+      wg_mma_n<W / 16, false>(acc[h], wg_desc_lo(smA + h * 64 * 128) + 2 * k, hi, wg_desc_lo(smB + c0 * 128) + 2 * k, hi, 8,
+                              k > 0 ? 1u : 0u);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc<W / 2>(acc[0]);
+  wg_fence_acc<W / 2>(acc[1]);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; h++)
+#pragma unroll
+    for (int e = 0; e < 2; e++) {
+      const int row = h * 64 + warp * 16 + (lane >> 2) + 8 * e;
+      const int ho = th * ST_TH + (row >> 4), wo = tw * ST_TW + (row & 15);
+      if (ho >= a.Ho || wo >= a.Wo) continue;
+      __half* o = a.out + ((size_t)(n * a.Ho + ho) * a.Wo + wo) * a.out_pitch + a.out_coff + c0;
+#pragma unroll
+      for (int J = 0; J < W / 8; J++) {
+        const int c = 8 * J + 2 * (lane & 3);
+        *reinterpret_cast<__half2*>(o + c) = __floats2half2_rn(silu_tanh(acc[h][4 * J + 2 * e] + s_bias[c0 + c]),
+                                                               silu_tanh(acc[h][4 * J + 2 * e + 1] + s_bias[c0 + c + 1]));
+      }
+    }
+}
+
 template <int DT>
 __global__ void __launch_bounds__(ST_THREADS, 4) stem_tc_kernel(const __grid_constant__ StemArgs a) {
   extern __shared__ __align__(1024) uint8_t st_smem[];
-  __shared__ __align__(8) uint64_t bars[2];  // a_ready, mma_done
-  __shared__ uint32_t tmem_slot;
   __shared__ __align__(16) float s_bias[256];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
+  const int tid = threadIdx.x;
   const uint32_t base = (smem_u32(st_smem) + 1023u) & ~1023u;
   const uint32_t smA = base;              // 128 rows x 128 B
   const uint32_t smB = base + 16 * 1024;  // Cout rows x 128 B
-  const uint32_t a_ready = smem_u32(&bars[0]), mma_done = smem_u32(&bars[1]);
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  if (tid == 0) {
-    mbar_init(a_ready, 128);
-    mbar_init(mma_done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                 "r"(a.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   // weights -> smem with the SWIZZLE_128B pattern; the K padding of the A rows is zeroed once
   for (int i = tid; i < a.Cout * 8; i += ST_THREADS) {
     const int n = i >> 3, pc = i & 7;
@@ -1338,106 +1045,60 @@ __global__ void __launch_bounds__(ST_THREADS, 4) stem_tc_kernel(const __grid_con
   }
   for (int i = tid; i < 128 * 8; i += ST_THREADS) st_shared_v4(smA + i * 16, make_int4(0, 0, 0, 0));
   for (int i = tid; i < a.Cout; i += ST_THREADS) s_bias[i] = a.bias[i];
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
   asm volatile("griddepcontrol.wait;" ::: "memory");
 
   const int tiles_per_img = a.tiles_w * a.tiles_h;
-  if (warp == 4) {
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(a.Cout >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      const uint32_t hi = 64u | (1u << 14) | (2u << 29);  // SBO = 8 rows x 128 B, version 1, SWIZZLE_128B
-      const uint32_t a_lo = ((smA & 0x3FFFF) >> 4) | (1u << 16), b_lo = ((smB & 0x3FFFF) >> 4) | (1u << 16);
-      int it = 0;
-      for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, it++) {
-        mbar_wait(a_ready, it & 1);
-        tc_fence_after();
-        umma_f16(tmem, desc64(a_lo, hi), desc64(b_lo, hi), idesc, 0);
-        umma_f16(tmem, desc64(a_lo + 2, hi), desc64(b_lo + 2, hi), idesc, 1);
-        umma_f16(tmem, desc64(a_lo + 4, hi), desc64(b_lo + 4, hi), idesc, 1);
-        umma_commit(mma_done);
+  const int tx = tid & (ST_TW - 1), ty = tid / ST_TW;  // output pixel of this thread's A row
+  const size_t plane = (size_t)a.src_H * a.src_W;
+  const bool ragged = a.src_W != a.W || a.src_H != a.H;  // padded source: rows may be misaligned and end early
+  const uint32_t pad1 = a.pad_h2 & 0xffffu;
+  auto gather = [&](int tile, uint2 (&v)[9]) {
+    const int n = fdiv(tile, a.m_tpi), r = tile - n * tiles_per_img;
+    const int th = fdiv(r, a.m_tw);
+    const int ho = th * ST_TH + ty, wo = (r - th * a.tiles_w) * ST_TW + tx;
+    const bool pix_ok = ho < a.Ho && wo < a.Wo;
+    const int col = 2 * wo - 2;
+#pragma unroll
+    for (int kh = 0; kh < 3; kh++) {
+      const int hi_ = ho * 2 + kh - 1;
+      const bool row_ok = pix_ok && hi_ >= 0 && hi_ < a.H;
+      const bool in_src = hi_ < a.src_H;
+      const size_t rowbase = (size_t)n * 3 * plane + (size_t)((row_ok && in_src) ? hi_ : 0) * a.src_W;
+#pragma unroll
+      for (int c = 0; c < 3; c++) {
+        uint2 g = make_uint2(0u, 0u);
+        if (row_ok) {
+          if (!ragged) g = stem_load4<DT>(a.in, rowbase + c * plane, col, wo > 0);
+          else if (in_src) g = stem_load4_ragged<DT>(a.in, rowbase + c * plane, col, a.src_W, pad1);
+          else g = make_uint2(wo > 0 ? a.pad_h2 : 0u, a.pad_h2);  // a row of the bottom padding
+        }
+        v[kh * 3 + c] = g;
       }
     }
-  } else {
-    const int tx = tid & (ST_TW - 1), ty = tid / ST_TW;  // output pixel inside the tile
-    const size_t plane = (size_t)a.src_H * a.src_W;
-    const bool ragged = a.src_W != a.W || a.src_H != a.H;  // padded source: rows may be misaligned and end early
-    const uint32_t pad1 = a.pad_h2 & 0xffffu;
-    auto gather = [&](int tile, uint2 (&v)[9]) {
-      const int n = fdiv(tile, a.m_tpi), r = tile - n * tiles_per_img;
-      const int th = fdiv(r, a.m_tw);
-      const int ho = th * ST_TH + ty, wo = (r - th * a.tiles_w) * ST_TW + tx;
-      const bool pix_ok = ho < a.Ho && wo < a.Wo;
-      const int col = 2 * wo - 2;
+  };
+  uint2 v[9];
+  if (blockIdx.x < a.total_tiles) gather(blockIdx.x, v);
+  const uint32_t a_row = smA + tid * 128;
+  const uint32_t sw = (uint32_t)(tid & 7);
+  for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
+    const int n = fdiv(tile, a.m_tpi), r = tile - n * tiles_per_img;
+    const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
+    __syncthreads();  // the previous tile's MMAs have retired in every warp before its A rows are overwritten
 #pragma unroll
-      for (int kh = 0; kh < 3; kh++) {
-        const int hi_ = ho * 2 + kh - 1;
-        const bool row_ok = pix_ok && hi_ >= 0 && hi_ < a.H;
-        const bool in_src = hi_ < a.src_H;
-        const size_t rowbase = (size_t)n * 3 * plane + (size_t)((row_ok && in_src) ? hi_ : 0) * a.src_W;
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-          uint2 g = make_uint2(0u, 0u);
-          if (row_ok) {
-            if (!ragged) g = stem_load4<DT>(a.in, rowbase + c * plane, col, wo > 0);
-            else if (in_src) g = stem_load4_ragged<DT>(a.in, rowbase + c * plane, col, a.src_W, pad1);
-            else g = make_uint2(wo > 0 ? a.pad_h2 : 0u, a.pad_h2);  // a row of the bottom padding
-          }
-          v[kh * 3 + c] = g;
-        }
+    for (int pc = 0; pc < 4; pc++)
+      st_shared_v4(a_row + ((pc ^ sw) << 4), make_int4((int)v[2 * pc].x, (int)v[2 * pc].y, (int)v[2 * pc + 1].x, (int)v[2 * pc + 1].y));
+    st_shared_v4(a_row + ((4u ^ sw) << 4), make_int4((int)v[8].x, (int)v[8].y, 0, 0));
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the MMA
+    __syncthreads();
+    if (tile + (int)gridDim.x < a.total_tiles) gather(tile + gridDim.x, v);  // next tile's loads fly during the MMA
+    for (int c0 = 0; c0 < a.Cout; c0 += 64) {
+      switch (min(64, a.Cout - c0)) {
+        case 64: stem_pass<64>(a, smA, smB, s_bias, c0, n, th, tw); break;
+        case 48: stem_pass<48>(a, smA, smB, s_bias, c0, n, th, tw); break;
+        case 32: stem_pass<32>(a, smA, smB, s_bias, c0, n, th, tw); break;
+        default: stem_pass<16>(a, smA, smB, s_bias, c0, n, th, tw); break;
       }
-    };
-    uint2 v[9];
-    if (blockIdx.x < a.total_tiles) gather(blockIdx.x, v);
-    const uint32_t a_row = smA + tid * 128;
-    const uint32_t sw = (uint32_t)(tid & 7);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, it++) {
-      const int n = fdiv(tile, a.m_tpi), r = tile - n * tiles_per_img;
-      const int th = fdiv(r, a.m_tw);
-      const int ho = th * ST_TH + ty, wo = (r - th * a.tiles_w) * ST_TW + tx;
-#pragma unroll
-      for (int pc = 0; pc < 4; pc++)
-        st_shared_v4(a_row + ((pc ^ sw) << 4), make_int4((int)v[2 * pc].x, (int)v[2 * pc].y, (int)v[2 * pc + 1].x, (int)v[2 * pc + 1].y));
-      st_shared_v4(a_row + ((4u ^ sw) << 4), make_int4((int)v[8].x, (int)v[8].y, 0, 0));
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the MMA
-      mbar_arrive(a_ready);
-      if (tile + (int)gridDim.x < a.total_tiles) gather(tile + gridDim.x, v);  // next tile's loads fly during the MMA
-      mbar_wait(mma_done, it & 1);
-      tc_fence_after();
-      const bool valid = ho < a.Ho && wo < a.Wo;
-      __half* o = a.out + ((size_t)(n * a.Ho + ho) * a.Wo + wo) * a.out_pitch + a.out_coff;
-      const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
-      for (int c0 = 0; c0 < a.Cout; c0 += 16) {
-        uint32_t acc[16];
-        tmem_ld16(taddr + c0, acc);
-        tmem_ld_wait();
-        if (valid) {
-          int4 o0, o1;
-          __half2* p0 = reinterpret_cast<__half2*>(&o0);
-          __half2* p1 = reinterpret_cast<__half2*>(&o1);
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            p0[j] = __floats2half2_rn(silu_tanh(__uint_as_float(acc[2 * j]) + s_bias[c0 + 2 * j]),
-                                      silu_tanh(__uint_as_float(acc[2 * j + 1]) + s_bias[c0 + 2 * j + 1]));
-            p1[j] = __floats2half2_rn(silu_tanh(__uint_as_float(acc[8 + 2 * j]) + s_bias[c0 + 8 + 2 * j]),
-                                      silu_tanh(__uint_as_float(acc[8 + 2 * j + 1]) + s_bias[c0 + 8 + 2 * j + 1]));
-          }
-          *reinterpret_cast<int4*>(o + c0) = o0;
-          *reinterpret_cast<int4*>(o + c0 + 8) = o1;
-        }
-      }
-      tc_fence_before();  // TMEM reads done before the next tile's MMA overwrites the accumulator
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(a.tmem_cols) : "memory");
   }
 }
 
@@ -1468,9 +1129,6 @@ int launch_stem_f16(const void* in, int in_dtype, int B, int H, int W, const __h
   a.total_tiles = B * a.tiles_w * a.tiles_h;
   auto magic = [](int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); };
   a.m_tpi = magic(a.tiles_w * a.tiles_h); a.m_tw = magic(a.tiles_w);
-  uint32_t cols = 32;
-  while (cols < (uint32_t)a.Cout) cols <<= 1;
-  a.tmem_cols = cols;
   static int num_sms = 0;
   const size_t smem = 1024 + 16 * 1024 + (size_t)a.Cout * 128;
   if (!num_sms) {
@@ -1481,8 +1139,7 @@ int launch_stem_f16(const void* in, int in_dtype, int B, int H, int W, const __h
     YB_CUDA_CHECK(cudaFuncSetAttribute(stem_tc_kernel<YB_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     YB_CUDA_CHECK(cudaFuncSetAttribute(stem_tc_kernel<YB_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
   }
-  const int per_sm = std::max(1, std::min(4, (int)(512 / cols)));
-  const int grid = std::min(a.total_tiles, num_sms * per_sm);
+  const int grid = std::min(a.total_tiles, num_sms * 4);
   if (in_dtype == YB_U8) stem_tc_kernel<YB_U8><<<grid, ST_THREADS, smem, s>>>(a);
   else if (in_dtype == YB_F16) stem_tc_kernel<YB_F16><<<grid, ST_THREADS, smem, s>>>(a);
   else stem_tc_kernel<YB_F32><<<grid, ST_THREADS, smem, s>>>(a);

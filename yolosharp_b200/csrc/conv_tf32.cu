@@ -1,4 +1,4 @@
-// Tensor-core convolutions of the TRAINING step (fp32 storage, TF32 tcgen05 MMAs, fp32 accumulate in TMEM).
+// Tensor-core convolutions of the TRAINING step (fp32 storage, TF32 MMAs, fp32 accumulate in registers).
 //
 // Replaces, on the training path, what libtorch runs behind `Conv2d.forward` and `loss.backward()` for the Conv
 // blocks of the reference (Modules/Convs.cs:44; Utils/Amp.cs:260-286 calls forward / backward / optimizer.step):
@@ -12,19 +12,20 @@
 //                    rectangle of one image, or 128 consecutive positions of the flattened batch for 1x1), N = output
 //                    channels (tile <= 256), K = taps x input channels.  Both operands K-major: A = NHWC activations
 //                    (one 4-D TMA box per tap and 32-channel slab, zero fill = padding, traversal stride = conv
-//                    stride), B = weights re-packed per step as [tap][N][K] (3-D TMA box).  A launch is described
+//                    stride), B = weights re-packed per step as [tap][N][K] (3-D TMA box); wgmma m64nNk8 TF32 from
+//                    two consumer warpgroups (64 rows each), one producer warp.  A launch is described
 //                    by a TAP TABLE (box offset dh, dw + weight slab per tap), which covers
 //                      forward          out(y,x) = sum_t in(y*s + kh - p, x*s + kw - p) W[kh][kw]
 //                      dgrad, stride 1  dx(y,x)  = sum_t dz(y + p - kh, x + p - kw) W^T[kh][kw]
 //                      dgrad, stride 2  four launches, one per output parity (py, px), each with the taps whose
 //                                       (py + p - kh) and (px + p - kw) are even, writing every second position
 //   tf_wgrad_kernel  dW[co][tap][ci] = sum_pixels dz[pix][co] * x[pix + tap][ci]: K = pixels, so both operands are
-//                    MN-major - exactly the NHWC tiles TMA delivers (64 pixels x 32 channels, 128-byte rows, written
-//                    with SWIZZLE_128B_ATOM_32B: the one shared-memory layout tcgen05 accepts for MN-major 32-bit
-//                    operands, UMMA layout type SWIZZLE_128B_BASE32B).  One CTA
-//                    owns 128 output channels x (taps x 32 nb) input channels in TMEM (<= 512 columns), walks its share
-//                    of the pixel tiles (split-K over pixels) and stores a partial; a fixed-order fold sums the
-//                    partials into the checkpoint layout (deterministic, no atomics).
+//                    MN-major - exactly the NHWC tiles TMA delivers (64 pixels x 32 channels, 128-byte SWIZZLE_128B
+//                    rows).  wgmma reads TF32 operands K-major only, so eight warps run mma.sync m16n8k8 TF32 with
+//                    fragments loaded from the swizzled tiles.  One CTA owns 128 output channels x (taps x 32 nb) input
+//                    channels (<= 128 accumulator columns, 64 registers per thread), walks its share of the pixel tiles
+//                    (split-K over pixels) and stores a partial; a fixed-order fold sums the partials into the
+//                    checkpoint layout (deterministic, no atomics).
 #include <cuda.h>
 
 #include <algorithm>
@@ -55,27 +56,17 @@ static TfEncodeFn tf_encode_fn() {
   return fn;
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ uint64_t tf_desc(uint32_t saddr, uint32_t lbo16, uint32_t sbo16, uint32_t layout) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)lbo16 << 16) | ((uint64_t)sbo16 << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)layout << 61);
-}
-
 constexpr int TF_MAX_STAGES = 8;
-constexpr int TF_THREADS = 192;  // warp 0 TMA producer, warp 1 MMA issuer (+ TMEM alloc), warps 2-5 epilogue
+constexpr int TF_CONSUMER_WARPS = 8;                      // two warpgroups (tf_conv_kernel) / eight MMA warps (wgrad)
+constexpr int TF_THREADS = 32 * TF_CONSUMER_WARPS + 32;  // + warp 8: TMA producer
+// blocks of the stem wgrad: a fixed count, so that the partials and their fold order (and the result) do not depend on the GPU
+constexpr int ST_WG_BLOCKS = 592;
 
 // ------------------------------------------------------------------------------------------
 // forward / data gradient
@@ -97,41 +88,57 @@ struct TfArgs {
   int BK;
   int stages;
   uint32_t a_stride, b_stride, a_bytes, b_bytes;
-  uint32_t layout, sbo16;
-  uint32_t tmem_cols;
+  uint32_t layout, sbo16;  // wgmma layout type (1 = SWIZZLE_128B, 2 = 64B, 3 = 32B), 8-row group stride >> 4
 };
 
-__global__ void __launch_bounds__(TF_THREADS, 2) tf_conv_kernel(const __grid_constant__ TfArgs a) {
-  // the barrier / TMEM setup below overlaps the tail of the previous kernel (launch_pdl); pdl_wait() before any global access
+template <int NT16, int KK>
+__device__ __forceinline__ void tf_mainloop(const TfArgs& a, float* acc, uint32_t smemA, uint32_t smemB, uint32_t full0, uint32_t empty0,
+                                            int& st, uint32_t& ph) {
+  const uint32_t hi = wg_desc_hi(a.sbo16, a.layout);
+  const uint32_t a_off = (threadIdx.x >> 7) * 8 * a.sbo16;  // warpgroup 1: rows 64.. = 8 groups of 8 rows further
+  const bool leader = (threadIdx.x & 31) == 0;
+  const int ksteps = a.ntaps * a.chunks;
+  uint32_t pend = 0;  // slot read by the previous commit group
+  for (int ks = 0; ks < ksteps; ks++) {
+    mbar_wait(full0 + 8 * st, ph);
+    const uint32_t a_lo = wg_desc_lo(smemA + st * a.a_stride) + a_off, b_lo = wg_desc_lo(smemB + st * a.b_stride);
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < KK; k++)  // 8 fp32 = 32 bytes per K step inside the swizzled row
+      wg_mma_n<NT16, true>(acc, a_lo + 2 * k, hi, b_lo + 2 * k, hi, KK * 2, (ks > 0 || k > 0) ? 1u : 0u);
+    wg_commit();
+    wg_wait<1>();
+    __syncwarp();
+    if (leader && pend) mbar_arrive(pend);
+    pend = empty0 + 8 * st;
+    if (++st == a.stages) { st = 0; ph ^= 1; }
+  }
+  wg_wait<0>();
+  __syncwarp();
+  if (leader && pend) mbar_arrive(pend);
+  wg_fence_acc<NT16 * 8>(acc);
+}
+
+template <int NT16>
+__global__ void __launch_bounds__(TF_THREADS, NT16 <= 4 ? 2 : 1) tf_conv_kernel(const __grid_constant__ TfArgs a) {
+  // the barrier setup below overlaps the tail of the previous kernel (launch_pdl); pdl_wait() before any global access
   extern __shared__ __align__(1024) uint8_t tf_smem[];
-  __shared__ __align__(8) uint64_t bars[2 * TF_MAX_STAGES + 4];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t bars[2 * TF_MAX_STAGES];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t smem0 = (smem_u32(tf_smem) + 1023u) & ~1023u;
   const uint32_t smemA = smem0, smemB = smem0 + a.stages * a.a_stride;
   const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[TF_MAX_STAGES]);
-  const uint32_t tfull0 = smem_u32(&bars[2 * TF_MAX_STAGES]), tempty0 = smem_u32(&bars[2 * TF_MAX_STAGES + 2]);
   if (threadIdx.x == 0) {
-    for (int s = 0; s < a.stages; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-    for (int s = 0; s < 2; s++) { mbar_init(tfull0 + 8 * s, 1); mbar_init(tempty0 + 8 * s, 4); }
+    for (int s = 0; s < a.stages; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, TF_CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(a.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_wait();
   pdl_trigger();
-  const uint32_t tmem_base = tmem_slot;
   const int tiles_per_img = a.tiles_w * a.tiles_h;
-  const int ksteps = a.ntaps * a.chunks;
 
-  if (warp == 0) {
+  if (warp == TF_CONSUMER_WARPS) {
     if (lane == 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmA) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmB) : "memory");
@@ -152,79 +159,42 @@ __global__ void __launch_bounds__(TF_THREADS, 2) tf_conv_kernel(const __grid_con
           }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // instruction descriptor: D fp32 (bit 4), A / B format TF32 (2 at bits 7 and 10), K-major both, N >> 3 at 17, M >> 4 at 24
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(a.n_tile >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      int st = 0, li = 0;
-      uint32_t ph = 0;
-      for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, li++) {
-        const int acc = li & 1;
-        mbar_wait(tempty0 + 8 * acc, ((uint32_t)(li >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * a.n_tile;
-        uint32_t accf = 0;
-        for (int ks = 0; ks < ksteps; ks++) {
-          mbar_wait(full0 + 8 * st, ph);
-          tc_fence_after();
-          const uint32_t sa = smemA + st * a.a_stride, sb = smemB + st * a.b_stride;
-          for (int k = 0; k < a.KK; k++) {  // 8 fp32 = 32 bytes per K step inside the swizzled row
-            umma_tf32(d_tmem, tf_desc(sa + 32 * k, 1, a.sbo16, a.layout), tf_desc(sb + 32 * k, 1, a.sbo16, a.layout), idesc, accf);
-            accf = 1;
-          }
-          umma_commit(empty0 + 8 * st);
-          if (++st == a.stages) { st = 0; ph ^= 1; }
-        }
-        umma_commit(tfull0 + 8 * acc);
-      }
-    }
   } else {
-    const int q = warp & 3;  // TMEM lane quarter this warp may read
-    const int row = q * 32 + lane;
-    int li = 0;
-    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, li++) {
-      const int acc = li & 1;
+    const int wg = warp >> 2, g = lane >> 2, t4 = lane & 3;
+    int st = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
+      float acc[NT16 * 8];
+      switch (a.KK) {
+        case 4: tf_mainloop<NT16, 4>(a, acc, smemA, smemB, full0, empty0, st, ph); break;
+        case 2: tf_mainloop<NT16, 2>(a, acc, smemA, smemB, full0, empty0, st, ph); break;
+        default: tf_mainloop<NT16, 1>(a, acc, smemA, smemB, full0, empty0, st, ph); break;
+      }
       const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
       const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
       const int th = r / a.tiles_w, tw = r - th * a.tiles_w;
-      const int hl = row / a.BW, wl = row - hl * a.BW;
-      const int ho = th * a.BH + hl, wo = tw * a.BW + wl;
-      const bool valid = hl < a.BH && ho < a.Ho && wo < a.Wo;
       const int n0 = nt * a.n_tile;
-      float* orow = a.out + (long long)img * a.o_img + (long long)ho * a.o_row + (long long)wo * a.o_pix + a.o_off + n0;
-      mbar_wait(tfull0 + 8 * acc, (uint32_t)(li >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * a.n_tile;
-      for (int c0 = 0; c0 < a.n_tile; c0 += 16) {
-        uint32_t v[16];
-        tmem_ld16(taddr + c0, v);
-        tmem_ld_wait();
-        if (valid) {
 #pragma unroll
-          for (int g = 0; g < 4; g++) {
-            const int c = n0 + c0 + g * 4;
-            if (c < a.n_out) {  // n_out is a multiple of 4
-              float4 o = make_float4(__uint_as_float(v[g * 4]), __uint_as_float(v[g * 4 + 1]), __uint_as_float(v[g * 4 + 2]),
-                                     __uint_as_float(v[g * 4 + 3]));
-              if (a.bias) {
-                const float4 b = *reinterpret_cast<const float4*>(a.bias + c);
-                o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w;
-              }
-              *reinterpret_cast<float4*>(orow + c0 + g * 4) = o;
+      for (int h = 0; h < 2; h++) {
+        const int row = wg * 64 + (warp & 3) * 16 + g + 8 * h;
+        const int hl = row / a.BW, wl = row - hl * a.BW;
+        const int ho = th * a.BH + hl, wo = tw * a.BW + wl;
+        if (hl >= a.BH || ho >= a.Ho || wo >= a.Wo) continue;
+        float* orow = a.out + (long long)img * a.o_img + (long long)ho * a.o_row + (long long)wo * a.o_pix + a.o_off + n0;
+#pragma unroll
+        for (int J = 0; J < NT16 * 2; J++) {
+          const int c = 8 * J + 2 * t4;
+          if (n0 + c < a.n_out) {  // n_out is a multiple of 4
+            float2 o = make_float2(acc[4 * J + 2 * h], acc[4 * J + 2 * h + 1]);
+            if (a.bias) {
+              const float2 b = *reinterpret_cast<const float2*>(a.bias + n0 + c);
+              o.x += b.x; o.y += b.y;
             }
+            *reinterpret_cast<float2*>(orow + c) = o;
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(a.tmem_cols) : "memory");
   }
 }
 
@@ -316,13 +286,13 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s) {
   a.chunks = (L.Kc + a.BK - 1) / a.BK;
   a.KK = a.BK / 8;
   const uint32_t row_bytes = a.BK * 4;
-  a.layout = a.BK == 32 ? 2 : (a.BK == 16 ? 4 : 6);
+  a.layout = a.BK == 32 ? 1 : (a.BK == 16 ? 2 : 3);
   a.sbo16 = (8 * row_bytes) >> 4;
   const CUtensorMapSwizzle swz = a.BK == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : (a.BK == 16 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
   a.n_tile = std::min(256, (L.Nc + 15) / 16 * 16);
   a.n_tiles = (L.Nc + a.n_tile - 1) / a.n_tile;
-  // (Tried: narrower N tiles for the 20 x 20 / 40 x 40 levels so that every SM gets a tile - 4.8 -> 5.1 ms over the step's
-  //  177 launches: the extra activation re-reads and shorter MMAs cost more than the idle SMs, profiles/r2_ncu_tf_conv.txt.)
+  // One N tile as wide as the layer: narrower tiles would give every SM a tile on the 20 x 20 / 40 x 40 levels, at the price
+  // of re-reading the activations once per N tile.
   cuuint64_t gdim[4], gstr[3];
   cuuint32_t box[4], estr[4];
   if (L.flat) {
@@ -367,27 +337,25 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s) {
   a.b_bytes = (uint32_t)a.n_tile * row_bytes;
   a.a_stride = (128 * row_bytes + 1023) / 1024 * 1024;
   a.b_stride = (a.n_tile * row_bytes + 1023) / 1024 * 1024;
-  uint32_t cols = 32;
-  while (cols < (uint32_t)(2 * a.n_tile)) cols <<= 1;
-  a.tmem_cols = cols;
-  // Two CTAs per SM when there are tiles for them and a CTA fits half an SM (<= 256 TMEM columns, a ring of >= 3 stages in
-  // ~100 KiB): with one producer thread, one MMA thread and four epilogue warps per CTA the kernel is latency bound
-  // (ncu: issue active 10 - 18 %, long-scoreboard / wait stalls, profiles/r2_ncu_tf_conv_big.txt); a second CTA fills
+  // Two CTAs per SM when there are tiles for them and a CTA fits half an SM (n_tile <= 64: 32 accumulator registers per
+  // thread, a ring of >= 3 stages in ~100 KiB): the consumers stall in the epilogue of every tile, and a second CTA fills
   // the other's load -> MMA -> epilogue bubbles, as in conv_tc_kernel.
   static const bool occ1 = getenv("YB_TF_OCC1") != nullptr;
   const size_t per_stage = (size_t)a.a_stride + a.b_stride;
   int occ = 1;
-  if (!occ1 && cols <= 256 && (size_t)(100 * 1024) / per_stage >= 3 && a.total_tiles >= 2 * tf_num_sms()) occ = 2;
+  if (!occ1 && a.n_tile <= 64 && (size_t)(100 * 1024) / per_stage >= 3 && a.total_tiles >= 2 * tf_num_sms()) occ = 2;
   a.stages = (int)std::min<size_t>(TF_MAX_STAGES, (size_t)((occ == 2 ? 100 : 190) * 1024) / per_stage);
   if (a.stages < 2) { set_error("tf32 conv: tile does not fit in shared memory"); return YB_ERR_SHAPE; }
   const size_t smem = (size_t)a.stages * (a.a_stride + a.b_stride) + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(tf_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set = true;
+  void (*kernel)(TfArgs) = nullptr;
+  dispatch_nt16(a.n_tile / 16, [&](auto nt16) { kernel = tf_conv_kernel<decltype(nt16)::value>; });
+  static bool attr_set[17] = {};
+  if (!attr_set[a.n_tile / 16]) {
+    YB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    attr_set[a.n_tile / 16] = true;
   }
   const int grid = std::min(a.total_tiles, occ * tf_num_sms());
-  YB_CUDA_CHECK(launch_pdl(tf_conv_kernel, dim3(grid), dim3(TF_THREADS), smem, s, a));
+  YB_CUDA_CHECK(launch_pdl(kernel, dim3(grid), dim3(TF_THREADS), smem, s, a));
   return 0;
 }
 
@@ -488,46 +456,45 @@ struct WgArgs {
   int tpc, tap_groups;  // taps per CTA (3 = one kh row of a 3x3, 1 for 1x1) and groups of them
   int imgs, tiles_w, tiles_h, pix_tiles;
   int b_stages;
-  int merge_kw;     // halo mode with one 32-channel input block: the three kw taps of a row as ONE N = 96 MMA
   int halo;         // 3x3 stride 1: ONE PH x (PW+2) input tile per pixel tile serves the three taps of a kh row (row-shifted windows)
   uint32_t xblk;    // bytes reserved per 32-channel block of an x stage (1 KiB aligned)
   int co_pad, ci_pad;
-  uint32_t tmem_cols;
 };
+
+// fp32 element (row r, channel c < 32) of a 128-byte-row SWIZZLE_128B tile whose base is 1 KiB aligned
+__device__ __forceinline__ uint32_t wg_ld(uint32_t base, int r, int c) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(base + r * 128 + ((((c >> 2) ^ (r & 7)) << 4) | ((c & 3) << 2))));
+  return v;
+}
+__device__ __forceinline__ void mma_tf32_16x8x8(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
 
 __global__ void __launch_bounds__(TF_THREADS, 1) tf_wgrad_kernel(const __grid_constant__ WgArgs a) {
   extern __shared__ __align__(1024) uint8_t wg_smem[];
-  __shared__ __align__(8) uint64_t bars[2 * WG_A_STAGES + 2 * 16 + 1];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t bars[2 * WG_A_STAGES + 2 * 16];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t smem0 = (smem_u32(wg_smem) + 1023u) & ~1023u;
   const uint32_t a_stride = 4 * WG_BLK, b_stride = (uint32_t)a.nb * a.xblk;
   const uint32_t smemA = smem0, smemB = smem0 + WG_A_STAGES * a_stride;
   const uint32_t afull = smem_u32(&bars[0]), aempty = smem_u32(&bars[WG_A_STAGES]);
   const uint32_t bfull = smem_u32(&bars[2 * WG_A_STAGES]), bempty = smem_u32(&bars[2 * WG_A_STAGES + 16]);
-  const uint32_t done = smem_u32(&bars[2 * WG_A_STAGES + 32]);
   if (threadIdx.x == 0) {
-    for (int s = 0; s < WG_A_STAGES; s++) { mbar_init(afull + 8 * s, 1); mbar_init(aempty + 8 * s, 1); }
-    for (int s = 0; s < a.b_stages; s++) { mbar_init(bfull + 8 * s, 1); mbar_init(bempty + 8 * s, 1); }
-    mbar_init(done, 1);
+    for (int s = 0; s < WG_A_STAGES; s++) { mbar_init(afull + 8 * s, 1); mbar_init(aempty + 8 * s, TF_CONSUMER_WARPS); }
+    for (int s = 0; s < a.b_stages; s++) { mbar_init(bfull + 8 * s, 1); mbar_init(bempty + 8 * s, TF_CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(a.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  // rows of the dz stages that are never loaded (Cout < 128) must not hold NaN bit patterns: 0 * NaN would poison nothing
-  // (every accumulator row depends on its own A row only), but keep the tensor pipe away from denormal/NaN slow paths
+  // rows of the dz stages that are never loaded (Cout < 128) feed accumulator rows that are never stored; zero them anyway
+  // so that no NaN / denormal bit patterns reach the tensor cores
   for (uint32_t i = threadIdx.x; i < WG_A_STAGES * a_stride / 16; i += TF_THREADS) st_shared_v4(smemA + i * 16, make_int4(0, 0, 0, 0));
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_wait();
   pdl_trigger();
-  const uint32_t tmem_base = tmem_slot;
 
   // CTA -> (output-channel tile, input-channel tile, pixel split)
   const int split = blockIdx.x % a.splits;
@@ -539,7 +506,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_wgrad_kernel(const __grid_co
   const int my_tiles = split < a.pix_tiles ? (a.pix_tiles - split + a.splits - 1) / a.splits : 0;
   const int ncols = a.nb * 32;  // accumulator columns per tap
 
-  if (warp == 0) {
+  if (warp == TF_CONSUMER_WARPS) {
     if (lane == 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmDz) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmX) : "memory");
@@ -578,106 +545,75 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_wgrad_kernel(const __grid_co
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // D fp32, A / B TF32, BOTH MN-major (bits 15, 16): operands are [pixel][channel] tiles, K runs over pixels
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(ncols >> 3) << 17) |
-                             ((uint32_t)(128 >> 4) << 24);
-      // MN-major 32-bit operands have ONE legal shared-memory layout: 128-byte rows (32 channels of one pixel) swizzled
-      // in 32-byte units over groups of 4 rows (UMMA layout type 1 = SWIZZLE_128B_BASE32B, written by TMA's
-      // SWIZZLE_128B_ATOM_32B).  LBO = next 32-channel block, SBO = next group of 4 pixels (K atoms of 4).
-      const uint32_t lbo16 = WG_BLK >> 4, sbo16 = 512 >> 4;
-      int sa = 0, sb = 0;
-      uint32_t pa = 0, pb = 0;
-      for (int i = 0; i < my_tiles; i++) {
-        mbar_wait(afull + 8 * sa, pa);
-        tc_fence_after();
-        const uint32_t A0 = smemA + sa * a_stride;
-        const uint32_t xlbo16 = a.xblk >> 4;
-        if (a.halo) {
-          mbar_wait(bfull + 8 * sb, pb);
-          tc_fence_after();
-          const uint32_t B0 = smemB + sb * b_stride;
-          if (a.merge_kw) {
-            // one 32-channel input block: the three kw windows are the SAME box shifted by one pixel row (128 bytes), so they
-            // are three N blocks of one MMA with a block stride (LBO) of 128 bytes - N = 96 instead of three N = 32 MMAs
-            // (a TF32 M = 128 MMA costs ~100 cycles whatever its N: the Cin <= 32 layers at 160 x 160 were MMA-issue bound)
-            const uint32_t idesc3 = (idesc & ~(0x3fu << 17)) | ((uint32_t)(96 >> 3) << 17);
-#pragma unroll
-            for (int ks = 0; ks < WG_PH; ks++)
-              umma_tf32(tmem_base, tf_desc(A0 + ks * 1024, lbo16, sbo16, 1),
-                        tf_desc(B0 + (uint32_t)(ks * (WG_PW + 2)) * 128, 128 >> 4, sbo16, 1), idesc3, (i > 0 || ks > 0) ? 1u : 0u);
-          } else {
-            for (int kw = 0; kw < 3; kw++) {
-              const uint32_t d_tmem = tmem_base + kw * ncols;
-#pragma unroll
-              for (int ks = 0; ks < WG_PH; ks++)  // output row ks: its 8 input pixels start at row ks * (PW + 2) + kw of the box
-                umma_tf32(d_tmem, tf_desc(A0 + ks * 1024, lbo16, sbo16, 1),
-                          tf_desc(B0 + (uint32_t)(ks * (WG_PW + 2) + kw) * 128, xlbo16, sbo16, 1), idesc, (i > 0 || ks > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(bempty + 8 * sb);
-          if (++sb == a.b_stages) { sb = 0; pb ^= 1; }
-        } else {
-          for (int tt = 0; tt < a.tpc; tt++) {
-            mbar_wait(bfull + 8 * sb, pb);
-            tc_fence_after();
-            const uint32_t B0 = smemB + sb * b_stride;
-            const uint32_t d_tmem = tmem_base + tt * ncols;
-#pragma unroll
-            for (int ks = 0; ks < WG_PW * WG_PH / 8; ks++)  // 8 pixels (K = 8) = 1 KiB = two 4-row swizzle atoms per block
-              umma_tf32(d_tmem, tf_desc(A0 + ks * 1024, lbo16, sbo16, 1), tf_desc(B0 + ks * 1024, xlbo16, sbo16, 1), idesc,
-                        (i > 0 || ks > 0) ? 1u : 0u);
-            umma_commit(bempty + 8 * sb);
-            if (++sb == a.b_stages) { sb = 0; pb ^= 1; }
-          }
-        }
-        umma_commit(aempty + 8 * sa);
-        if (++sa == WG_A_STAGES) { sa = 0; pa ^= 1; }
-      }
-      umma_commit(done);
-    }
   } else {
-    const int q = warp & 3;
-    const int co = co_t * 128 + q * 32 + lane;
-    if (my_tiles > 0) {
-      mbar_wait(done, 0);
-      tc_fence_after();
-    }
-    float* prow = a.part + (((size_t)split * a.co_pad + co) * a.taps) * a.ci_pad + (size_t)ci_t * ncols;
-    for (int tt = 0; tt < a.tpc; tt++)
-      for (int c0 = 0; c0 < ncols; c0 += 16) {
-        const int t = tap0 + tt;
-        uint32_t v[16];
-        if (my_tiles > 0) {
-          tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + tt * ncols + c0, v);
-          tmem_ld_wait();
-        } else {
+    // warp w: output channels 16w .. 16w+15 of the CTA's 128 (A rows) and every accumulator column; column block j (8
+    // columns) is tap j / (nb * 4), input channels 8 * (j % (nb * 4)) ..  At most 128 columns: 16 blocks x 4 registers.
+    const int g = lane >> 2, t4 = lane & 3;
+    const int nblk = a.tpc * a.nb * 4;
+    const int acol = 16 * (warp & 1) + g;  // channel of this lane's A rows inside 32-channel block warp / 2
+    float acc[16][4];
 #pragma unroll
-          for (int j = 0; j < 16; j++) v[j] = 0u;
-        }
-        if (co < a.Cout) {
+    for (int j = 0; j < 16; j++) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+    int sa = 0, sb = 0;
+    uint32_t pa = 0, pb = 0;
+    const int nst = a.halo ? 1 : a.tpc;  // B stages per pixel tile
+    for (int i = 0; i < my_tiles; i++) {
+      mbar_wait(afull + 8 * sa, pa);
+      const uint32_t A0 = smemA + sa * a_stride + (warp >> 1) * WG_BLK;
+      uint32_t B0[3];
 #pragma unroll
-          for (int g = 0; g < 4; g++)
-            *reinterpret_cast<float4*>(prow + (size_t)t * a.ci_pad + c0 + g * 4) =
-                make_float4(__uint_as_float(v[g * 4]), __uint_as_float(v[g * 4 + 1]), __uint_as_float(v[g * 4 + 2]),
-                            __uint_as_float(v[g * 4 + 3]));
+      for (int q = 0; q < 3; q++) {
+        const int sq = sb + q < a.b_stages ? sb + q : sb + q - a.b_stages;
+        if (q < nst) mbar_wait(bfull + 8 * sq, sb + q < a.b_stages ? pb : (pb ^ 1));
+        B0[q] = smemB + (q < nst ? sq : sb) * b_stride;
+      }
+      for (int ks = 0; ks < WG_PW * WG_PH / 8; ks++) {  // 8 pixels = one pixel row of the tile per K step
+        uint32_t af[4];
+        af[0] = wg_ld(A0, 8 * ks + t4, acol);
+        af[1] = wg_ld(A0, 8 * ks + t4, acol + 8);
+        af[2] = wg_ld(A0, 8 * ks + t4 + 4, acol);
+        af[3] = wg_ld(A0, 8 * ks + t4 + 4, acol + 8);
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+          if (j < nblk) {
+            const int tt = a.tpc == 3 ? (j >> 2) : 0, jj = a.tpc == 3 ? (j & 3) : j;  // tpc = 3 implies nb = 1
+            const uint32_t bb = (a.halo ? B0[0] : B0[tt]) + (jj >> 2) * a.xblk;
+            // halo: output row ks reads input pixels ks * (PW + 2) + kw .. of the box
+            const int r0 = a.halo ? ks * (WG_PW + 2) + t4 + tt : 8 * ks + t4;
+            const int c = (jj & 3) * 8 + g;
+            mma_tf32_16x8x8(acc[j], af, wg_ld(bb, r0, c), wg_ld(bb, r0 + 4, c));
+          }
         }
       }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(a.tmem_cols) : "memory");
+      __syncwarp();  // every lane's shared-memory reads of this tile are done
+      if (lane == 0) {
+        mbar_arrive(aempty + 8 * sa);
+        for (int q = 0; q < nst; q++) mbar_arrive(bempty + 8 * (sb + q < a.b_stages ? sb + q : sb + q - a.b_stages));
+      }
+      if (++sa == WG_A_STAGES) { sa = 0; pa ^= 1; }
+      for (int q = 0; q < nst; q++)
+        if (++sb == a.b_stages) { sb = 0; pb ^= 1; }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int co = co_t * 128 + warp * 16 + g + 8 * h;
+      if (co >= a.Cout) continue;
+      float* prow = a.part + (((size_t)split * a.co_pad + co) * a.taps) * a.ci_pad + (size_t)ci_t * ncols;
+#pragma unroll
+      for (int j = 0; j < 16; j++) {
+        if (j < nblk) {
+          const int tt = a.tpc == 3 ? (j >> 2) : 0, jj = a.tpc == 3 ? (j & 3) : j;
+          *reinterpret_cast<float2*>(prow + (size_t)(tap0 + tt) * a.ci_pad + 8 * jj + 2 * t4) = make_float2(acc[j][2 * h], acc[j][2 * h + 1]);
+        }
+      }
+    }
   }
 }
 
 // dw[co][ci][tap] = sum over splits (fixed order) of part[split][co][tap][ci]
 // One block per output channel: the partials are read along ci (coalesced), summed over the splits in split order, transposed
 // through shared memory ([ci][tap], stride `taps` is odd or 1: no bank conflicts) and written as the contiguous run
-// dw[co][:][:].  (Threads over the checkpoint layout read 4-byte words ci_pad apart: 0.86 ms over the 79 folds of a YOLOv11s
-// step; reads coalesced over ci with scattered writes: 1.13 ms.)
+// dw[co][:][:].  (Threads over the checkpoint layout would read 4-byte words ci_pad apart.)
 __global__ void __launch_bounds__(256) tf_wgrad_fold_kernel(const float* __restrict__ part, float* __restrict__ dw, int Cout, int Cin,
                                                             int taps, int splits, int co_pad, int ci_pad) {
   pdl_wait();
@@ -710,10 +646,10 @@ static WgPlan wg_plan(int N, int H, int W, int Cin, int Cout, int k, int stride,
   const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
   const int taps = k * k;
   const int ci_blocks = (Cin + 31) / 32;
-  // a CTA owns 128 output channels x (tpc taps x nb * 32 input channels) in TMEM: tpc = 3 (one kh row of a 3x3) x up to
-  // 128 channels = 384 columns.  (The first version kept all nine taps of 32 input channels: N = 32 per MMA, and a
-  // TF32 M=128 MMA costs ~110 cycles whatever its N - 8.7 % tensor activity, profiles/r2_ncu_tf_wgrad.txt.)
-  p.nb = std::min(ci_blocks, 4);
+  // a CTA owns 128 output channels x (tpc taps x nb * 32 input channels) of accumulators in registers, at most 128
+  // columns: tpc = 3 (one kh row of a 3x3) x 32 channels, or one tap x up to 128 channels
+  p.tpc = taps == 9 ? 3 : 1;
+  p.nb = std::min(ci_blocks, p.tpc == 3 ? 1 : 4);
   p.ci_tiles = (ci_blocks + p.nb - 1) / p.nb;
   p.co_tiles = (Cout + 127) / 128;
   p.co_pad = p.co_tiles * 128;
@@ -721,11 +657,10 @@ static WgPlan wg_plan(int N, int H, int W, int Cin, int Cout, int k, int stride,
   p.tiles_w = (Wo + WG_PW - 1) / WG_PW;
   p.tiles_h = (Ho + WG_PH - 1) / WG_PH;
   p.pix_tiles = N * p.tiles_w * p.tiles_h;
-  p.tpc = taps == 9 ? 3 : 1;
   p.tap_groups = taps / p.tpc;
   const int pairs = p.co_tiles * p.ci_tiles * p.tap_groups;
   // pixel splits: one CTA per SM (189 KiB of shared memory), so the grid should fill ONE wave of SMs, or two when that fills
-  // them noticeably better - never a few CTAs over (ceil(2 * 148 / pairs) capped at 64 gave grids of 300 - 320 = a third
+  // them noticeably better - never a few CTAs over (ceil(2 * SMs / pairs) capped at 64 gave grids of 300 - 320 = a third
   // wave of 4 - 24 CTAs on a third of the layers, and 64-CTA grids on the 1x1 layers with <= 128 channels)
   const int sms = tf_num_sms();
   const int s1 = std::max(1, sms / pairs), s2 = std::max(1, 2 * sms / pairs);
@@ -739,7 +674,7 @@ size_t tf_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, in
   const WgPlan p = wg_plan(N, H, W, Cin, Cout, k, stride, k / 2);
   const size_t part = (size_t)p.splits * p.co_pad * k * k * p.ci_pad * 4;
   const size_t wpk = (size_t)Cout * Cin * k * k * 4;
-  return std::max(std::max(part, wpk), (size_t)148 * 4 * 27 * 128 * sizeof(float)) + 256;
+  return std::max(std::max(part, wpk), (size_t)ST_WG_BLOCKS * 27 * 128 * sizeof(float)) + 256;
 }
 
 int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
@@ -763,27 +698,20 @@ int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W
   a.imgs = N; a.tiles_w = p.tiles_w; a.tiles_h = p.tiles_h; a.pix_tiles = p.pix_tiles;
   a.co_pad = p.co_pad; a.ci_pad = p.ci_pad;
   // 3x3 stride 1: the input tile with its halo is loaded once per pixel tile and the nine taps are row-shifted MMA windows
-  // into it (the per-tap form moved 9 x 8 KiB of x per 64 pixels and was bound by L2 -> SM delivery).  The shifted start
-  // relies on tcgen05 applying the 32-byte-atom swizzle on absolute shared-memory address bits, as the K-major halo tile
-  // of conv_tc.cu does for the 16-byte-atom modes; tests/test_gpu_conv_tc.py's bit-exact case covers it.
+  // into it (the per-tap form moved 9 x 8 KiB of x per 64 pixels and was bound by L2 -> SM delivery).
   static const bool no_halo = getenv("YB_WGRAD_NO_HALO") != nullptr;
   a.halo = (k == 3 && stride == 1 && !no_halo) ? 1 : 0;
-  static const bool no_merge = getenv("YB_WGRAD_NO_MERGE") != nullptr;
-  a.merge_kw = (a.halo && p.nb == 1 && !no_merge) ? 1 : 0;
   a.xblk = a.halo ? (uint32_t)(((WG_PW + 2) * WG_PH * 128 + 1023) / 1024 * 1024) : (uint32_t)WG_BLK;
   const size_t b_stride = (size_t)p.nb * a.xblk;
   a.b_stages = (int)std::min<size_t>(16, ((size_t)190 * 1024 - (size_t)WG_A_STAGES * 4 * WG_BLK) / b_stride);
   if (a.b_stages < 2) { set_error("tf32 wgrad: tile does not fit in shared memory"); return YB_ERR_SHAPE; }
-  uint32_t cols = 32;
-  while (cols < (uint32_t)(a.tpc * p.nb * 32)) cols <<= 1;
-  a.tmem_cols = cols;
   {
     cuuint64_t gd[4] = {(cuuint64_t)Cout, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)N};
     cuuint64_t gs[3] = {(cuuint64_t)Cout * 4, (cuuint64_t)Cout * 4 * Wo, (cuuint64_t)Cout * 4 * Wo * Ho};
     cuuint32_t bx[4] = {32, WG_PW, WG_PH, 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
     CUresult cr = encode(&a.tmDz, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(dz), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) { set_error("tf32 wgrad: cuTensorMapEncodeTiled(dz) failed with code " + std::to_string((int)cr)); return YB_ERR_CUDA; }
   }
   {
@@ -792,7 +720,7 @@ int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W
     cuuint32_t bx[4] = {32, (cuuint32_t)(a.halo ? WG_PW + 2 : WG_PW * stride), (cuuint32_t)(a.halo ? WG_PH : WG_PH * stride), 1};
     cuuint32_t es[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
     CUresult cr = encode(&a.tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) { set_error("tf32 wgrad: cuTensorMapEncodeTiled(x) failed with code " + std::to_string((int)cr)); return YB_ERR_CUDA; }
   }
   static bool attr_set = false;
@@ -819,9 +747,8 @@ int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W
 
 // ------------------------------------------------------------------------------------------
 // The 3-channel stem (model.0: Conv(3, C, k = 3, s = 2), Yolo.cs:53) on CUDA cores, fp32.
-// On the tensor-core path the stem ran with its input zero-padded to 8 channels: K = 8 per tap means one tiny MMA per TMA
-// box of 128 strided 32-byte rows, and both passes were bound by the TMA row rate - forward 239 us and wgrad 1 288 us of a
-// 24.6 ms step (profiles/r2_ncu_tf_conv_big.txt, r2_ncu_tf_wgrad_big.txt), for 0.3 % of the step's FLOPs.  Here:
+// On the tensor cores the stem would need its input zero-padded to 8 channels: K = 8 per tap means one tiny MMA per TMA
+// box of 128 strided 32-byte rows, bound by the TMA row rate, for 0.3 % of the step's FLOPs.  Here:
 //   forward   one thread per output pixel and 32-channel group: its 27 inputs in registers, weights [27][C] in shared memory
 //   wgrad     dW[co][ci][kh][kw] = sum over pixels of dz[p][co] * x[window(p)][ci][kh][kw]: a block stages 128 pixels (their
 //             27-value windows and dz rows) in shared memory, thread (co lane, tap group) accumulates its share of the
@@ -879,8 +806,8 @@ __global__ void __launch_bounds__(256) stem3_forward_kernel(const float* __restr
 // as [kh][column][4] (one 16-byte load per input pixel, coalesced), so the 3 x 3 window of output pixel p is 3 x three
 // adjacent float4 of shared memory; dz of the tile is staged as [pixel][C].  Thread = (channel lane, warp g): warp g takes
 // pixels g, g + 8, ... and keeps all 27 taps of its channel(s) in registers: per pixel 9 broadcast LDS.128 + 1 LDS feed
-// 27 FMAs (the first version staged im2col windows element by element - ~40 integer instructions per staged value - and
-// spent 5 LDS per 4 FMAs: 690 us for 1.4 GFMA).  The 8 warps are folded in warp order through shared memory, the blocks'
+// 27 FMAs (staging im2col windows element by element costs ~40 integer instructions per staged value and 5 LDS per
+// 4 FMAs).  The 8 warps are folded in warp order through shared memory, the blocks'
 // partials by stem3_wgrad_fold_kernel in block order: deterministic.
 // grid.x blocks walk the tiles with stride gridDim.x; partial[block][27][C], k = (kh * 3 + kw) * 3 + ci
 template <int CG>  // 32-channel groups per thread: ceil(C / 32)
@@ -974,16 +901,16 @@ int stem3_forward(const float* x, int xc, const float* w, int N, int H, int W, i
   if (C % 8 || C > 128 || (H & 1) || (W & 1) || xc < 3) { set_error("stem conv: C % 8 == 0, C <= 128, even input size"); return YB_ERR_SHAPE; }
   const int Ho = H / 2, Wo = W / 2;
   const long long total = (long long)N * Ho * Wo * ((C + 31) / 32);
-  const int grid = (int)std::min<long long>((total + 255) / 256, 148 * 16);
+  const int grid = (int)std::min<long long>((total + 255) / 256, tf_num_sms() * 16);
   stem3_forward_kernel<<<grid, 256, (size_t)27 * C * sizeof(float), s>>>(x, xc, w, z, N, H, W, Ho, Wo, C);
   YB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
-size_t stem3_wgrad_workspace_bytes(int C) { return (size_t)148 * 4 * 27 * C * sizeof(float); }
+size_t stem3_wgrad_workspace_bytes(int C) { return (size_t)ST_WG_BLOCKS * 27 * C * sizeof(float); }
 int stem3_backward_weight(const float* x, int xc, const float* dz, int N, int H, int W, int C, float* dw, float* ws, size_t ws_bytes,
                           cudaStream_t s) {
   if (C % 8 || C > 128 || (H & 1) || (W & 1) || xc < 3) { set_error("stem wgrad: C % 8 == 0, C <= 128, even input size"); return YB_ERR_SHAPE; }
-  const int blocks = 148 * 4;
+  const int blocks = ST_WG_BLOCKS;
   if (ws_bytes < stem3_wgrad_workspace_bytes(C)) { set_error("stem wgrad: workspace too small"); return YB_ERR_INVALID_ARG; }
   const int Ho = H / 2, Wo = W / 2;
   const size_t smem = (size_t)(3 * (2 * ST_PIX + 1) * 4 + std::max(ST_PIX * C, 8 * 27 * 32)) * sizeof(float);

@@ -71,7 +71,7 @@ struct OpDesc {
   int lane_level = -1; // pyramid level whose feature map a side lane waits for
   int feat_level = -1; // this op completes feats[feat_level] (fork point for the head lanes)
   int dep_op = -1;     // layer chaining: the op whose per-image completion gates this op's tiles (-1: whole previous grid)
-  EpiDecode dec;       // conv: fused Detect-tail epilogue (tcgen05 path)
+  EpiDecode dec;       // conv: fused Detect-tail epilogue (tensor-core path)
   bool fused = false;  // decode op: its work is done by the producing convs' epilogues
 };
 
@@ -173,7 +173,7 @@ struct Builder {
 
   // Several Conv modules that read the SAME input (the first convs of the Detect branches, Head.cs:47-49)
   // as one conv whose output channels are the concatenation of theirs: one pass over the input and a
-  // wider N per tcgen05.mma (N = 144 instead of 64 and 80).
+  // wider N per wgmma (N = 144 instead of 64 and 80).
   void conv_merged(const std::vector<std::string>& names, const std::vector<int>& couts, VRef in, VRef out, int k, int s) {
     OpDesc op;
     op.type = OP_CONV;
@@ -646,7 +646,7 @@ static int finalize_conv(yb_engine* e, OpDesc& op) {
         wg[((size_t)t * op.cin + ci) * op.cout + o] = wf[((size_t)o * op.cin + ci) * taps + t];
   if (upload(e, wg, &op.w_f32)) return YB_ERR_CUDA;
   if (f16) {
-    // tensor-core layout [Cout][tap][Cin] (K-major rows for the UMMA B operand)
+    // tensor-core layout [Cout][tap][Cin] (K-major rows for the wgmma B operand)
     std::vector<__half> wh((size_t)op.cout * taps * op.cin);
     for (int o = 0; o < op.cout; o++)
       for (int t = 0; t < taps; t++)
@@ -696,7 +696,7 @@ static int run_ops(yb_engine* e, const void* in, int in_dtype, int B, float* out
   int rc;
   bool input_converted = false;
   // Head branches are independent chains of small, latency-bound kernels: with every Detect tail fused
-  // (tcgen05 path) they run on side streams forked at the op that completes their feature map and are
+  // (tensor-core path) they run on side streams forked at the op that completes their feature map and are
   // joined at the end; inside a captured CUDA graph this becomes real branch parallelism.
   const bool lanes = e->lanes_ok && !events && only < 0;
   bool lane_started[yb_engine::kLanes] = {};
@@ -811,7 +811,7 @@ extern "C" {
 int32_t yb_abi_version(void) { return YB_ABI_VERSION; }
 
 const char* yb_build_info(void) {
-  return "yolob200 (sm_100a; tcgen05+TMA conv, CUDA-core fp32 parity path) built " __DATE__ " " __TIME__;
+  return "yolob200 (sm_90a; wgmma+TMA conv, CUDA-core fp32 parity path) built " __DATE__ " " __TIME__;
 }
 
 const char* yb_last_error(void) { return g_last_error.c_str(); }
@@ -845,8 +845,8 @@ int32_t yb_create(const yb_config* cfg, yb_engine** out) {
   YB_CUDA_CHECK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   YB_CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) {
-    set_error(std::string("yb_create: device '") + prop.name + "' is not sm_100 (Blackwell B200); this library only contains sm_100a code");
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error(std::string("yb_create: device '") + prop.name + "' is not sm_90 (Hopper H100); this library only contains sm_90a code");
     return YB_ERR_NO_DEVICE;
   }
   std::unique_ptr<yb_engine> e(new yb_engine());
@@ -854,7 +854,7 @@ int32_t yb_create(const yb_config* cfg, yb_engine** out) {
   e->esize = cfg->precision == YB_PREC_F16 ? 2 : 4;
   int rc = build_graph(e.get());
   if (rc) return rc;
-  // workspace: one arena, every buffer sized for max_batch, 1 KiB aligned (TMA/UMMA friendly)
+  // workspace: one arena, every buffer sized for max_batch, 1 KiB aligned (TMA / wgmma friendly)
   size_t off = 0;
   for (auto& b : e->bufs) {
     b.offset = off;
@@ -969,7 +969,7 @@ int32_t yb_finalize_weights(yb_engine* e) {
   const bool f16 = e->cfg.precision == YB_PREC_F16;
   const bool allow_tc = f16 && !(e->cfg.flags & YB_FLAG_NO_TCGEN05);
   if (allow_tc) {
-    // Detect tail fusion: when every final 1x1 conv of a level can run on the tcgen05 kernel, their
+    // Detect tail fusion: when every final 1x1 conv of a level can run on the tensor-core kernel, their
     // epilogues write the prediction tensor directly and the decode kernel is dropped.
     for (auto& d : e->ops) {
       if (d.type != OP_DECODE) continue;
@@ -1012,7 +1012,7 @@ int32_t yb_finalize_weights(yb_engine* e) {
       if (tc_conv_supported(p)) {
         std::string err;
         op.plan = tc_conv_plan_create(p, &err);
-        if (!op.plan) { set_error("tcgen05 plan failed for " + op.name + ": " + err); return YB_ERR_CUDA; }
+        if (!op.plan) { set_error("tensor-core plan failed for " + op.name + ": " + err); return YB_ERR_CUDA; }
         op.use_tc = true;
         if (getenv("YB_DEBUG_PLANS")) fprintf(stderr, "[plan] %-30s k%d s%d %4d->%4d @%dx%d  %s\n", op.name.c_str(), op.k, op.s, op.cin, op.cout,
                                               p.Ho, p.Wo, tc_conv_plan_describe(op.plan).c_str());
@@ -1023,11 +1023,11 @@ int32_t yb_finalize_weights(yb_engine* e) {
     if (d.type != OP_DECODE || !d.fused) continue;
     for (auto& c : e->ops)
       if (c.type == OP_CONV && c.dec.mode != EPI_STORE && c.dec.a0 == d.a0 && !c.use_tc) {
-        set_error("internal: fused decode producer " + c.name + " did not get a tcgen05 plan");
+        set_error("internal: fused decode producer " + c.name + " did not get a tensor-core plan");
         return YB_ERR_STATE;
       }
   }
-  // Layer chaining: inside a lane, a tcgen05 conv whose stream predecessor is a tcgen05 conv that stores an NHWC
+  // Layer chaining: inside a lane, a tensor-core conv whose stream predecessor is a tensor-core conv that stores an NHWC
   // tensor starts its tiles per image, as soon as the predecessor has stored that image (per-image counters), instead
   // of waiting for the predecessor's whole grid.  Completion per image is monotone along the lane (every op waits for
   // its predecessor's image before it stores its own), so the predecessor's counter also covers older producers of the
@@ -1485,7 +1485,7 @@ int32_t yb_op_cost(const yb_engine* e, int32_t i, int32_t batch, double* flops, 
   return YB_OK;
 }
 
-/* debug: the `skip`-th tcgen05 conv launch from now on records a timeline (CTA 0: MMA-issuer and first
+/* debug: the `skip`-th tensor-core conv launch from now on records a timeline (CTA 0: MMA-issuer and first
  * epilogue warp clock64 stamps for its first 16 tiles) into dev_buf (128 x int64). */
 int32_t yb_debug_timeline(long long* dev_buf, int32_t skip) {
   yb::g_tc_dbg = dev_buf;

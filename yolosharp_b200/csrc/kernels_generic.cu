@@ -1,6 +1,6 @@
 // CUDA-core kernels of the yolob200 engine, templated on the activation storage type.
 //   T = float  : parity mode (fp32 storage, fp32 FMA) - matches the fp32 oracle to ~1e-5
-//   T = __half : debug twin of the tcgen05 path (same fp16 storage/weights, fp32 accumulate)
+//   T = __half : debug twin of the tensor-core path (same fp16 storage/weights, fp32 accumulate)
 // plus the HBM-bound glue ops used by both modes (SPPF pool, upsample, decode, layout).
 // Reference ops restated: Modules/Convs.cs:36-56 (Conv), Block.cs:236-282 (SPPF),
 // Head.cs:204-223 + Block.cs:15-45 + Utils/Tal.cs:313-356 (decode).
@@ -167,8 +167,7 @@ __global__ void dwconv3x3_kernel(ConvParams p, size_t total) {
 // fp16 path, channels in groups of 8 (one 16-byte vector): a thread produces DW_PIX adjacent output pixels of one row
 // for 8 channels from a 3 x (DW_PIX + 2) window of 16-byte loads (4.5 loads per output instead of 9 scalar ones), the
 // 72 weights of its channel group in registers.  Consecutive threads = consecutive channel groups: every load / store
-// instruction of a warp covers whole contiguous pixel rows.  (The scalar kernel above ran the YOLOv11 head's depthwise
-// convs at 4 % of the HBM roofline: 1.2 ms of the 4.7 ms YOLOv11s forward at batch 32.)
+// instruction of a warp covers whole contiguous pixel rows.  (The scalar kernel above issues 9 scalar loads per output.)
 constexpr int DW_PIX = 4;
 __global__ void __launch_bounds__(256) dwconv3x3_h8_kernel(ConvParams p, int groups8, int wtiles, int total) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -766,9 +765,8 @@ __global__ void __launch_bounds__(256) attention_kernel(View qkv, View out, View
 
 // Tiled variant for kd = 32, hd = 64 (all YOLOv11 sizes), used when a head's K and V fit in shared memory (N <= 416
 // tokens: every 640 x 640 model).  The row kernel above re-streams K and V through shared memory for every 8 query rows
-// (6 400 CTAs x 77 KB and 100 block-wide barriers each for YOLOv11s at batch 32: 0.88 ms, 19 % of the forward).  A first
-// tiled version with scalar shared-memory reads was no faster (1.0 ms): three LDS per two FMAs made it shared-memory
-// bound.  This one is register-blocked:
+// (6 400 CTAs x 77 KB and 100 block-wide barriers each for YOLOv11s at batch 32).  Scalar shared-memory reads would
+// make a tiled version shared-memory bound (three LDS per two FMAs).  This one is register-blocked:
 //   * a CTA (16 warps) owns 32 query rows of one (head, image); K (row stride 36 floats) and V (stride 64) stay resident as fp32
 //   * scores: a warp owns 2 query rows, held in 64 registers; a lane owns one key per block of 32 and reads its K row
 //     with 8 conflict-free LDS.128 -> 64 FMAs per 8 loads
@@ -839,8 +837,7 @@ __global__ void __launch_bounds__(ATI_THREADS, 1) attention_tiled_32x64_kernel(A
     }
   }
   // the dense copy of v that the positional-encoding conv reads: this CTA's 32 rows, one vector per thread.  (Inside the
-  // fill loop above these stores sat between the batched loads and each waited for its own load: 45 % of the kernel's
-  // stall samples, profiles/r2_ncu_attention_tiled.txt.)
+  // fill loop above these stores would sit between the batched loads and each wait for its own load.)
   if (vo) {
     const int r = threadIdx.x >> 4, d = (threadIdx.x & 15) * 4, j = i0 + r;
     if (j < N) cp4<T>(vo + (size_t)b * io.out_img + (size_t)j * io.out_tok + head * ATI_HD + d, vb + (size_t)j * io.v_tok + d);

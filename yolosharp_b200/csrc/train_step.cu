@@ -6,7 +6,7 @@
 // AdamW over flat parameter buffers.  The graph walk that `yolosharp_b200/train.py` / `train_v11.py` do in Python over
 // the library's kernels lives here in C++ over the same kernels (the Python steps stay as the executable specification
 // this file is tested against, tests/test_trainer_native.py):
-//   dense convolutions   TF32 tcgen05 forward / dgrad / wgrad (csrc/conv_tf32.cu); the 3-channel stem runs with its
+//   dense convolutions   TF32 tensor-core forward / dgrad / wgrad (csrc/conv_tf32.cu); the 3-channel stem runs with its
 //                        input zero-padded to 8 channels
 //   BatchNorm + SiLU     csrc/bn_train.cu (batch statistics, running-stat update, backward)
 //   depthwise 3x3, attention   csrc/train_v11.cu
@@ -1119,7 +1119,7 @@ int32_t yb_trainer_create(const yb_config* cfg, yb_trainer** out) {
   {
     // the kernels' scratch (BatchNorm partials, attention statistics, ...) comes from the stream-ordered allocator; by
     // default its pool hands unused memory back to the OS at every synchronisation - and a step ends with one (loss items
-    // to the host) - so the next step would pay for fresh device allocations (seen as random 15 - 500 ms steps)
+    // to the host) - so the next step would pay for fresh device allocations (random slow steps)
     cudaMemPool_t pool;
     if (cudaDeviceGetDefaultMemPool(&pool, cfg->device) == cudaSuccess) {
       uint64_t keep = UINT64_MAX;

@@ -78,8 +78,8 @@ __global__ void __launch_bounds__(256) dw3x3_forward4_kernel(const float* __rest
 // 4 channels x 4 adjacent pixels of a row per thread: the 3 x 6 input window is loaded once (18 x 16 B, addresses clamped and
 // out-of-image values zeroed afterwards, so that no load is predicated and all are in flight together) and feeds four
 // outputs; the weights sit in shared memory as [tap][C].  Same fmaf chain per output element as the kernels above (taps
-// in kh, kw order; a zero-padded tap adds 0 * w).  The per-pixel kernel above spent 58 us per launch on the Detect
-// branches of YOLOv11s (9 predicated loads and 36 scalar weight loads per 4 outputs).
+// in kh, kw order; a zero-padded tap adds 0 * w).  The per-pixel kernel above needs 9 predicated loads and 36 scalar
+// weight loads per 4 outputs.
 __global__ void __launch_bounds__(256) dw3x3_forward_row4_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                                 float* __restrict__ z, int N, int H, int W, int C, int transpose_taps,
                                                                 int total) {
@@ -259,7 +259,7 @@ __global__ void __launch_bounds__(256) dw3x3_wgrad_partial4_kernel(const float* 
 }
 
 // fold of the slab partials with 8 lanes per (tap, channel): lane y adds slabs y, y + 8, ... in order, lanes added in order
-// (one thread walking 400 slabs serially was a 10 us dependent-load chain)
+// (one thread walking 400 slabs serially would be a long dependent-load chain)
 __global__ void __launch_bounds__(256) dw3x3_wgrad_fold8_kernel(const float* __restrict__ partial, float* __restrict__ dw, int slabs, int C) {
   __shared__ float f[8][32];
   const int i = blockIdx.x * 32 + threadIdx.x;  // (t, c)
@@ -477,7 +477,7 @@ __global__ void __launch_bounds__(AT_THREADS) attn_backward_kv_kernel(const floa
 // ---------------------------------------------------------------------------------------------------------------
 // Tiled attention (the path that runs for the network's shapes: N = 400 tokens at 640 x 640, kd = 32, hd = 64).
 // The row kernels above launch one CTA per (token, head, image) and every CTA streams the head's whole K and V from
-// L2 (25 600 CTAs x 150 KB for one YOLOv11s layer at batch 16: 13 ms forward + backward).  Here a CTA owns a tile of
+// L2 (25 600 CTAs x 150 KB for one YOLOv11s layer at batch 16).  Here a CTA owns a tile of
 // AT_T = 16 tokens of one (head, image) and keeps the head's K and V (or Q and dO) in shared memory:
 //   row strides kd + 1 / hd + 1 make both access patterns - lanes over tokens (score / dP dot products) and lanes
 //   over channels (P.V, dS.K accumulations) - bank-conflict free;  8 warps, two token rows per warp share every
@@ -497,7 +497,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 }
 // rows of one head of a (B, N, nh, dim) tensor -> shared memory with row stride `ld` (dim a multiple of 4, 16-byte aligned
 // rows in global memory).  Eight independent 16-byte loads are in flight per thread: with one CTA of 8 warps per SM a
-// load-store loop of scalar loads exposed the full L2 latency per element (the two backward kernels spent ~85 us per CTA).
+// load-store loop of scalar loads would expose the full L2 latency per element.
 __device__ __forceinline__ void load_head(float* dst, const float* src, int b, int h, int N, int nh, int dim, int ld, int row0,
                                           int rows) {
   constexpr int U = 8;

@@ -466,7 +466,7 @@ class ConvWorkspace:
 
 
 def conv_forward_tc(x, w, bias=None, stride=1, pad=None, ws=None, stream=None):
-    """yb_conv_forward_tc: x (N,H,W,Cin) NHWC float32, w (Cout,Cin,k,k) -> z (N,Ho,Wo,Cout); TF32 tcgen05 MMAs."""
+    """yb_conv_forward_tc: x (N,H,W,Cin) NHWC float32, w (Cout,Cin,k,k) -> z (N,Ho,Wo,Cout); TF32 tensor-core MMAs."""
     assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and w.is_cuda and w.dtype == torch.float32 and w.is_contiguous()
     N, H, W, Cin = x.shape
     Cout, _, k, _ = w.shape

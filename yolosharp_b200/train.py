@@ -9,7 +9,7 @@ of the graph (channel concat / chunk views, nearest 2x upsampling and its sum-re
 SPPF and its index backward - the last two are the remaining library calls on this path).
 
 This is the PARITY path of the training side: correct first (it matches autograd through the oracle restatement
-parameter by parameter), CUDA-core fp32 kernels; the tcgen05 dgrad / wgrad kernels and a captured train-mode graph
+parameter by parameter), CUDA-core fp32 kernels; the tensor-core dgrad / wgrad kernels and a captured train-mode graph
 replace it next.  Parameter names are the reference's state_dict keys (`model.{i}.conv.weight`, ...).
 """
 import math
@@ -59,7 +59,7 @@ class KernelOps:
     """The C-ABI kernels (no fallback: importing this on a machine without the CUDA library fails loudly)."""
 
     def __init__(self, tensor_cores=True):
-        """tensor_cores: dense convolutions (forward, dgrad, wgrad) on the TF32 tcgen05 kernels (csrc/conv_tf32.cu) where
+        """tensor_cores: dense convolutions (forward, dgrad, wgrad) on the TF32 tensor-core kernels (csrc/conv_tf32.cu) where
         their shape rule holds (channels % 8, k in {1, 3}); False = the fp32 CUDA-core parity kernels everywhere."""
         from . import engine as E
         self.E = E
