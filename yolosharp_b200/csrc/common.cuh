@@ -160,6 +160,14 @@ struct TcChain {
 int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cudaStream_t s, const TcChain* chain = nullptr);
 int tc_conv_rows_per_image(const TcConvPlan* plan);  // rows x N tiles one image contributes to done_ctr
 bool tc_conv_supported(const ConvParams& p);
+// Fused Bottleneck (DESIGN 4.1): the 3x3 conv `pa` and the 3x3 conv `pb` that reads its output (plus the shortcut
+// `pb` may carry) as one launch; the intermediate stays in shared memory.  Uses both plans' packed weights, so they must
+// outlive it.  nullptr (and *err) when the pair's shapes do not fit the kernel.
+struct TcBneckPlan;
+TcBneckPlan* tc_bneck_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, std::string* err);
+void tc_bneck_plan_destroy(TcBneckPlan* plan);
+std::string tc_bneck_plan_describe(const TcBneckPlan* plan);
+int tc_bneck_launch(const TcBneckPlan* plan, int B, int* tile_ctr, cudaStream_t s);
 // stem: NCHW u8/f16/f32 input -> 3x3 s2 conv (Cin=3) + bias + SiLU -> NHWC fp16
 int launch_stem_f16(const void* in, int in_dtype, int B, int H, int W, const __half* w16 /*[Cout][32]*/,
                     const float* bias, const View& out, cudaStream_t s, int src_H = 0, int src_W = 0);  // src_*: unpadded source size

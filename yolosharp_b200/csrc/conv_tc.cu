@@ -24,6 +24,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <vector>
 
 #include "common.cuh"
@@ -130,6 +131,23 @@ __device__ __forceinline__ int tq_get(const int* s_tile, const volatile int* s_h
   __threadfence_block();
   return reinterpret_cast<const volatile int*>(s_tile)[li & (TQ - 1)];
 }
+// The producer's tile sequence: blockIdx.x first, then batches of `batch` consecutive tiles from the launch's counter,
+// each drawn one batch ahead so that the atomic's latency never sits on the load path (ctr == nullptr: round-robin).
+struct TileDraw {
+  int tile, nxt, left, batch, total;
+  int* ctr;
+  __device__ __forceinline__ TileDraw(int* c, int b, int tot)
+      : tile((int)blockIdx.x), nxt(tot), left(1), batch(b), total(tot), ctr(c) {
+    if (ctr && tile < total) nxt = (int)gridDim.x + atomicAdd(ctr, batch);
+  }
+  __device__ __forceinline__ void advance() {
+    if (!ctr) { tile += gridDim.x; return; }
+    if (--left > 0) { tile++; return; }
+    tile = nxt;
+    left = batch;
+    if (tile < total) nxt = (int)gridDim.x + atomicAdd(ctr, batch);
+  }
+};
 
 // Producer-side dependency wait of the layer chain: poll the producer launch's counter of image `img` until all of
 // its rows are stored (acquire), bounded like every other wait of this kernel.
@@ -435,13 +453,10 @@ __global__ void __launch_bounds__(TC_THREADS, NT16 <= 4 ? 2 : 1) conv_tc_kernel(
       int sa = 0, sb = 0;
       uint32_t pa = 0, pb = 0;
       int li = 0;
-      int tile = (int)blockIdx.x;
-      int nxt = a.total_tiles, left = 1;
-      const int batch = a.tile_batch;
-      // the next batch of tiles is drawn one batch ahead, so the atomic's latency never sits on the load path
-      if (dyn && tile < a.total_tiles) nxt = (int)gridDim.x + atomicAdd(a.tile_ctr, batch);
+      TileDraw td(a.tile_ctr, a.tile_batch, a.total_tiles);
       int dep_ready = -1;  // last image of the producer known to be complete
-      for (; tile < a.total_tiles; li++) {
+      for (; td.tile < a.total_tiles; li++) {
+        const int tile = td.tile;
         if (a.dep_ctr != nullptr) {
           // images this tile reads: its own image, or for a flattened 1x1 tile the images of its first / last pixel
           const int mt0 = fdiv(tile, a.m_ntiles);
@@ -496,17 +511,7 @@ __global__ void __launch_bounds__(TC_THREADS, NT16 <= 4 ? 2 : 1) conv_tc_kernel(
             }
           }
         }
-        if (dyn) {
-          if (--left > 0) {
-            tile++;
-          } else {
-            tile = nxt;
-            left = batch;
-            if (tile < a.total_tiles) nxt = (int)gridDim.x + atomicAdd(a.tile_ctr, batch);
-          }
-        } else {
-          tile += gridDim.x;
-        }
+        td.advance();
       }
       if (dyn) tq_publish(s_tile, &s_head, li, -1);  // end mark
     }
@@ -891,6 +896,417 @@ int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cu
   cfg.attrs = attr;
   static const bool no_pdl = getenv("YB_DEBUG_NO_PDL") != nullptr;  // experiments only (tools/exp_fixed_cost.py)
   cfg.numAttrs = no_pdl ? 0 : 1;
+  YB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, plan->kernel, a));
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// Fused Bottleneck (Block.cs:572-607 with k = (3, 3)): out = SiLU(conv_b(t) + bias_b) [+ x], t = fp16(SiLU(conv_a(x) +
+// bias_a)).  t never leaves shared memory; the block input is read from HBM once and also serves as the shortcut.
+//   tile      the 8 x 16 output rectangle of a halo tile (HALO_BW x HALO_BH)
+//   input     one 4-D TMA box {BK1, 12, 20, 1} per channel slab at (w0 - 2, h0 - 2), zero out-of-bounds fill: box pixel
+//             (h, w) sits at row 12 h + w
+//   stage 1   M = box rows 0..255, four blocks of 64 (two per warpgroup), SBO = 8 rows: row 12 h + w is t pixel (h, w)
+//             of the 10 x 18 halo of t when w < 10 and h < 18, i.e. 180 of the 256 MMA rows do useful work.  Tap (kh, kw)
+//             is the same bytes shifted by 12 kh + kw rows (as TC_HALO); the rows that run past the box only feed the
+//             discarded MMA rows.
+//   t         fp16 in shared memory at the same row index (pitch 12), one slab per BK2 channels, swizzled as a TMA box of
+//             that width would be; zero where its pixel lies outside the image (the zero padding of conv_b)
+//   stage 2   the TC_HALO mapping over t with SBO = 12 rows, both weight sets resident
+//   shortcut  the centre of the staged input box, read into registers before its ring slot is handed back
+// Rounding points are those of the two unfused launches: fp32 sums, + bias, SiLU, fp16 t; the same for stage 2, then
+// + residual and the fp16 store.
+// ------------------------------------------------------------------------------------------
+constexpr int BN_PITCH = HALO_BW + 4;               // width of the input box = row pitch of t
+constexpr int BN_XROWS = BN_PITCH * (HALO_BH + 4);  // 240 rows of the input box
+constexpr int BN_TROWS = BN_PITCH * (HALO_BH + 2);  // 216 rows of t (columns 10 and 11 unused)
+constexpr int BN_MAX_C = 64;                        // cmid, cout: one N tile of at most 64 columns per stage
+constexpr size_t BN_MAX_RINGS = 220 * 1024;         // input ring + weights + t of a one-CTA-per-SM plan (+ 1 KiB alignment)
+
+struct BnArgs {
+  CUtensorMap tmX;
+  const uint8_t *w1, *w2;  // packed weight slabs of conv_a / conv_b (pack_weights_kernel, one N tile)
+  const float *bias1, *bias2;
+  __half* out;
+  int out_pitch, out_coff;
+  int shortcut;
+  int H, W, tiles_w, tiles_h, total_tiles;
+  uint64_t m_tpi, m_tw;
+  int cmid, cout;
+  int BK1, chunks1, BK2, chunks2;
+  uint32_t layout1, layout2;          // wgmma layout types of the BK1 / BK2 rows
+  uint32_t x_bytes, x_stride, slot;   // input: TMA bytes / smem bytes per channel slab; one ring slot = chunks1 slabs
+  uint32_t w1_bytes, w2_bytes, b1_stride, b2_stride;
+  uint32_t t_stride;                  // smem bytes per BK2-channel slab of t
+  int stages;
+  int* tile_ctr;
+  int tile_batch;
+};
+
+struct TcBneckPlan {
+  BnArgs args;
+  size_t smem;
+  int grid, occ;
+  void (*kernel)(BnArgs) = nullptr;
+};
+
+// byte offset of (row r, byte b) in a slab of `rb`-byte swizzled rows whose base is 1 KiB aligned (pack_weights_kernel)
+__device__ __forceinline__ uint32_t sw_off(uint32_t r, uint32_t b, uint32_t rb) {
+  const uint32_t sw = rb == 128 ? (r & 7) : (rb == 64 ? ((r >> 1) & 3) : ((r >> 2) & 1));
+  return r * rb + ((((b >> 4) ^ sw)) << 4) + (b & 15);
+}
+
+// stage 1 of one warpgroup: MMA rows 128 wg .. 128 wg + 127 as two 64-row accumulators, one commit group per tile
+template <int NM16, int KK>
+__device__ __forceinline__ void bn_stage1(const BnArgs& a, float (&acc)[2][NM16 * 8], uint32_t xslot, uint32_t w1, int wg) {
+  constexpr uint32_t RB16 = KK * 2;
+  const uint32_t hi = wg_desc_hi(8 * RB16, a.layout1);
+  uint32_t scale = 0;
+  wg_fence();
+  for (int ch = 0; ch < a.chunks1; ch++) {
+    const uint32_t a_lo = wg_desc_lo(xslot + ch * a.x_stride) + (uint32_t)wg * 128 * RB16;
+#pragma unroll
+    for (int t = 0; t < 9; t++) {
+      const uint32_t tap = (uint32_t)((t / 3) * BN_PITCH + t % 3) * RB16;
+      const uint32_t b_lo = wg_desc_lo(w1 + (t * a.chunks1 + ch) * a.b1_stride);
+#pragma unroll
+      for (int k = 0; k < KK; k++) {
+#pragma unroll
+        for (int j = 0; j < 2; j++) wg_mma_n<NM16, false>(acc[j], a_lo + j * 64 * RB16 + tap + 2 * k, hi, b_lo + 2 * k, hi, RB16, scale);
+        scale = 1;
+      }
+    }
+  }
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc<NM16 * 8>(acc[0]);
+  wg_fence_acc<NM16 * 8>(acc[1]);
+}
+
+// stage 2 of one warpgroup: output rows 64 wg.. (image rows 8 wg..) over t, SBO = one t row of 12 pixels
+template <int NO16, int KK>
+__device__ __forceinline__ void bn_stage2(const BnArgs& a, float* acc, uint32_t tbase, uint32_t w2, int wg) {
+  constexpr uint32_t RB16 = KK * 2;
+  const uint32_t a_hi = wg_desc_hi(BN_PITCH * RB16, a.layout2), b_hi = wg_desc_hi(8 * RB16, a.layout2);
+  uint32_t scale = 0;
+  wg_fence();
+  for (int ch = 0; ch < a.chunks2; ch++) {
+    const uint32_t a_lo = wg_desc_lo(tbase + ch * a.t_stride) + (uint32_t)wg * 8 * BN_PITCH * RB16;
+#pragma unroll
+    for (int t = 0; t < 9; t++) {
+      const uint32_t tap = (uint32_t)((t / 3) * BN_PITCH + t % 3) * RB16;
+      const uint32_t b_lo = wg_desc_lo(w2 + (t * a.chunks2 + ch) * a.b2_stride);
+#pragma unroll
+      for (int k = 0; k < KK; k++) {
+        wg_mma_n<NO16, false>(acc, a_lo + tap + 2 * k, a_hi, b_lo + 2 * k, b_hi, RB16, scale);
+        scale = 1;
+      }
+    }
+  }
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc<NO16 * 8>(acc);
+}
+
+// CTAs per SM the register bound of each instantiation allows without spills (ptxas -v): the per-tile chain of loads,
+// two MMA stages and two epilogues is latency-bound at small channel counts, so concurrent CTAs are what fills the SM
+__host__ __device__ constexpr int bn_ctas_per_sm(int nm16, int no16) { return nm16 == 1 && no16 <= 2 ? 3 : (nm16 <= 2 && no16 <= 2 ? 2 : 1); }
+
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(TC_CONSUMERS) : "memory"); }
+
+template <int NM16, int NO16>
+__global__ void __launch_bounds__(TC_THREADS, bn_ctas_per_sm(NM16, NO16)) bneck_tc_kernel(const __grid_constant__ BnArgs a) {
+  extern __shared__ __align__(1024) uint8_t bn_smem[];
+  __shared__ __align__(8) uint64_t bars[2 * TC_MAX_STAGES + 1];
+  __shared__ int s_tile[TQ];
+  __shared__ volatile int s_head;
+  __shared__ __align__(16) float s_bias1[BN_MAX_C], s_bias2[BN_MAX_C];
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < a.cmid; i += blockDim.x) s_bias1[i] = a.bias1[i];  // constant data
+  for (int i = threadIdx.x; i < a.cout; i += blockDim.x) s_bias2[i] = a.bias2[i];
+  const uint32_t sX = (smem_u32(bn_smem) + 1023u) & ~1023u;  // input ring, then W1, W2, t
+  const uint32_t sW1 = sX + a.stages * a.slot, sW2 = sW1 + a.w1_bytes, sT = sW2 + a.w2_bytes;
+  const uint32_t full = smem_u32(&bars[0]), empty = smem_u32(&bars[TC_MAX_STAGES]), wfull = smem_u32(&bars[2 * TC_MAX_STAGES]);
+  // t starts zeroed: when cmid is not a multiple of BK2 (48 channels in 64-channel slabs), channels cmid.. of every row
+  // are K padding that stage 2 multiplies with zero weights and the epilogue never writes - stale bytes there could be
+  // Inf / NaN patterns
+  for (uint32_t i = threadIdx.x; i < a.chunks2 * a.t_stride / 16; i += blockDim.x) st_shared_v4(sT + 16 * i, make_int4(0, 0, 0, 0));
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy zeros -> visible to the MMA
+
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if (warp == TC_CONSUMER_WARPS && lane == 0) {
+    s_head = 0;
+    for (int s = 0; s < a.stages; s++) {
+      mbar_init(full + 8 * s, 1);
+      mbar_init(empty + 8 * s, TC_CONSUMER_WARPS);
+    }
+    mbar_init(wfull, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+  if (warp == TC_CONSUMER_WARPS && lane == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmX) : "memory");
+    // weights do not depend on the previous kernel: fetch them before the grid dependency resolves
+    mbar_arrive_expect_tx(wfull, a.w1_bytes + a.w2_bytes);
+    bulk_load_1d(sW1, a.w1, a.w1_bytes, wfull);
+    bulk_load_1d(sW2, a.w2, a.w2_bytes, wfull);
+  }
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+
+  const int tiles_per_img = a.tiles_w * a.tiles_h;
+  if (warp == TC_CONSUMER_WARPS) {
+    // ===================== TMA producer: one ring slot (all input channel slabs) per tile =====================
+    if (lane == 0) {
+      int s = 0, li = 0;
+      uint32_t ph = 0;
+      TileDraw td(a.tile_ctr, a.tile_batch, a.total_tiles);
+      for (; td.tile < a.total_tiles; li++) {
+        const int tile = td.tile;
+        tq_publish(s_tile, &s_head, li, tile);
+        const int img = fdiv(tile, a.m_tpi), r = tile - img * tiles_per_img;
+        const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
+        mbar_wait(empty + 8 * s, ph ^ 1);
+        mbar_arrive_expect_tx(full + 8 * s, a.chunks1 * a.x_bytes);
+        for (int ch = 0; ch < a.chunks1; ch++)
+          tma_load_4d(sX + s * a.slot + ch * a.x_stride, &a.tmX, full + 8 * s, ch * a.BK1, tw * HALO_BW - 2, th * HALO_BH - 2, img);
+        if (++s == a.stages) { s = 0; ph ^= 1; }
+        td.advance();
+      }
+      tq_publish(s_tile, &s_head, li, -1);  // end mark
+    }
+    return;
+  }
+  // ===================== consumers =====================
+  const int wg = warp >> 2, g = lane >> 2, t4 = lane & 3;
+  const uint32_t rb1 = a.BK1 * 2, rb2 = a.BK2 * 2;
+  int s = 0;
+  uint32_t ph = 0;
+  mbar_wait(wfull, 0);
+  for (int li = 0;; li++) {
+    const int tile = tq_get(s_tile, &s_head, li);
+    if (tile < 0) break;
+    const int img = fdiv(tile, a.m_tpi), r = tile - img * tiles_per_img;
+    const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
+    const int h0 = th * HALO_BH, w0 = tw * HALO_BW;
+    const uint32_t xslot = sX + s * a.slot;
+    mbar_wait(full + 8 * s, ph);
+    float acc1[2][NM16 * 8];
+    switch (a.BK1) {
+      case 64: bn_stage1<NM16, 4>(a, acc1, xslot, sW1, wg); break;
+      case 32: bn_stage1<NM16, 2>(a, acc1, xslot, sW1, wg); break;
+      default: bn_stage1<NM16, 1>(a, acc1, xslot, sW1, wg); break;
+    }
+    // shortcut: this thread's stage-2 rows are box pixels (hl + 2, wl + 2); read before the slot is handed back
+    uint32_t res[2][NO16 * 2];
+    if (a.shortcut) {
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int row = wg * 64 + (warp & 3) * 16 + g + 8 * h;
+        const uint32_t xr = (uint32_t)(((row >> 3) + 2) * BN_PITCH + (row & 7) + 2);
+#pragma unroll
+        for (int J = 0; J < NO16 * 2; J++) {
+          const int c = 8 * J + 2 * t4;
+          res[h][J] = ld_shared_u32(xslot + (c / a.BK1) * a.x_stride + sw_off(xr, (c % a.BK1) * 2, rb1));
+        }
+      }
+      // these generic-proxy reads must be performed before the producer's TMA (async proxy) refills the slot
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty + 8 * s);
+    if (++s == a.stages) { s = 0; ph ^= 1; }
+    // t of the previous tile is free: every warpgroup retired its stage-2 MMAs before reaching this point
+    consumers_sync();
+#pragma unroll
+    for (int j = 0; j < 2; j++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int row = (2 * wg + j) * 64 + (warp & 3) * 16 + g + 8 * h;
+        const int hh = row / BN_PITCH, ww = row - hh * BN_PITCH;
+        if (row >= BN_TROWS || ww >= HALO_BW + 2) continue;
+        const int y = h0 - 1 + hh, x = w0 - 1 + ww;
+        const bool inside = y >= 0 && y < a.H && x >= 0 && x < a.W;
+#pragma unroll
+        for (int J = 0; J < NM16 * 2; J++) {
+          const int c = 8 * J + 2 * t4;
+          float f0 = 0.f, f1 = 0.f;
+          if (inside) {
+            const float2 b = *reinterpret_cast<const float2*>(s_bias1 + c);
+            f0 = silu_tanh(acc1[j][4 * J + 2 * h] + b.x);
+            f1 = silu_tanh(acc1[j][4 * J + 2 * h + 1] + b.y);
+          }
+          const __half2 v = __floats2half2_rn(f0, f1);
+          st_shared_u32(sT + (c / a.BK2) * a.t_stride + sw_off((uint32_t)row, (c % a.BK2) * 2, rb2),
+                        *reinterpret_cast<const uint32_t*>(&v));
+        }
+      }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy t writes -> visible to the MMA
+    consumers_sync();
+    float acc2[NO16 * 8];
+    switch (a.BK2) {
+      case 64: bn_stage2<NO16, 4>(a, acc2, sT, sW2, wg); break;
+      case 32: bn_stage2<NO16, 2>(a, acc2, sT, sW2, wg); break;
+      default: bn_stage2<NO16, 1>(a, acc2, sT, sW2, wg); break;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int row = wg * 64 + (warp & 3) * 16 + g + 8 * h;
+      const int y = h0 + (row >> 3), x = w0 + (row & 7);
+      if (y >= a.H || x >= a.W) continue;
+      __half* orow = a.out + ((size_t)(img * a.H + y) * a.W + x) * a.out_pitch + a.out_coff;
+#pragma unroll
+      for (int J = 0; J < NO16 * 2; J++) {
+        const int c = 8 * J + 2 * t4;
+        const float2 b = *reinterpret_cast<const float2*>(s_bias2 + c);
+        float f0 = silu_tanh(acc2[4 * J + 2 * h] + b.x), f1 = silu_tanh(acc2[4 * J + 2 * h + 1] + b.y);
+        if (a.shortcut) {
+          const float2 xv = __half22float2(*reinterpret_cast<const __half2*>(&res[h][J]));
+          f0 += xv.x; f1 += xv.y;
+        }
+        *reinterpret_cast<__half2*>(orow + c) = __floats2half2_rn(f0, f1);
+      }
+    }
+  }
+}
+
+TcBneckPlan* tc_bneck_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, std::string* err) {
+  const ConvParams &p1 = pa->p, &p2 = pb->p;
+  const TcArgs &a1 = pa->args, &a2 = pb->args;
+  auto fail = [&](const char* m) -> TcBneckPlan* { if (err) *err = m; return nullptr; };
+  if (a1.mode != TC_HALO || a2.mode != TC_HALO || a1.n_tiles != 1 || a2.n_tiles != 1 || p1.Cout != p2.Cin ||
+      p1.Cout > BN_MAX_C || p2.Cout > BN_MAX_C || p1.act != ACT_SILU || p2.act != ACT_SILU || p1.res.base ||
+      a1.epi_mode != EPI_STORE || a2.epi_mode != EPI_STORE)
+    return fail("not a fusable 3x3 / 3x3 pair");
+  const bool shortcut = p2.res.base != nullptr;
+  if (shortcut && (p2.res.base != p1.in.base || p2.res.coff != p1.in.coff || p2.res.pitch != p1.in.pitch || p1.Cin != p2.Cout))
+    return fail("shortcut is not the block input");
+  EncodeTiledFn encode = get_encode_fn(err);
+  if (!encode) return nullptr;
+  TcBneckPlan* plan = new TcBneckPlan();
+  BnArgs& a = plan->args;
+  memset(&a, 0, sizeof(a));
+  const size_t esz = 2;
+  cuuint64_t gdim[4] = {(cuuint64_t)p1.Cin, (cuuint64_t)p1.in.W, (cuuint64_t)p1.in.H, (cuuint64_t)p1.B};
+  cuuint64_t gstr[3];
+  gstr[0] = (cuuint64_t)p1.in.pitch * esz;
+  gstr[1] = gstr[0] * p1.in.W;
+  gstr[2] = gstr[1] * p1.in.H;
+  cuuint32_t box[4] = {(cuuint32_t)a1.BK, (cuuint32_t)BN_PITCH, (cuuint32_t)(HALO_BH + 4), 1}, estr[4] = {1, 1, 1, 1};
+  const CUtensorMapSwizzle swz = a1.BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (a1.BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+  CUresult cr = encode(&a.tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, reinterpret_cast<char*>(p1.in.base) + (size_t)p1.in.coff * esz,
+                       gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) {
+    delete plan;
+    return fail("cuTensorMapEncodeTiled(bottleneck input) failed");
+  }
+  a.w1 = a1.wpk; a.w2 = a2.wpk;
+  a.bias1 = p1.bias; a.bias2 = p2.bias;
+  a.out = reinterpret_cast<__half*>(p2.out.base);
+  a.out_pitch = p2.out.pitch; a.out_coff = p2.out.coff;
+  a.shortcut = shortcut;
+  a.H = p2.Ho; a.W = p2.Wo;
+  a.cmid = p1.Cout; a.cout = p2.Cout;
+  a.BK1 = a1.BK; a.chunks1 = a1.chunks; a.layout1 = a1.layout_a;
+  a.BK2 = a2.BK; a.chunks2 = a2.chunks; a.layout2 = a2.layout_a;
+  auto kib = [](size_t b) { return (uint32_t)((b + 1023) / 1024 * 1024); };
+  a.x_bytes = (uint32_t)(BN_XROWS * a.BK1 * 2);
+  a.x_stride = kib(a.x_bytes);
+  a.slot = a.chunks1 * a.x_stride;
+  a.b1_stride = a1.b_stride; a.b2_stride = a2.b_stride;
+  a.w1_bytes = (uint32_t)(a1.ksteps * a1.b_stride);
+  a.w2_bytes = (uint32_t)(a2.ksteps * a2.b_stride);
+  a.t_stride = kib((size_t)BN_TROWS * a.BK2 * 2);
+  const size_t fixed = (size_t)a.w1_bytes + a.w2_bytes + (size_t)a.chunks2 * a.t_stride;
+  // as many CTAs per SM as the kernel's register bound allows and their rings fit; otherwise one CTA with as deep an
+  // input ring as the remaining shared memory holds (one slot at c = 64: the input slot is handed back right after
+  // stage 1, so the next tile's load still overlaps stage 2)
+  const int nm16 = a.cmid / 16, no16 = a.cout / 16;
+  plan->occ = 0;
+  for (int occ = bn_ctas_per_sm(nm16, no16); occ >= 1 && !plan->occ; occ--) {
+    const size_t budget = occ == 3 ? 72 * 1024 : (occ == 2 ? 104 * 1024 : BN_MAX_RINGS);
+    if (fixed >= budget) continue;
+    a.stages = (int)std::min<size_t>(4, (budget - fixed) / a.slot);
+    if (a.stages >= occ) plan->occ = occ;
+  }
+  if (!plan->occ) {
+    delete plan;
+    return fail("bottleneck tile does not fit in shared memory");
+  }
+  // At one CTA per SM both stages and their epilogues run back to back with nothing to overlap them, and without a
+  // shortcut the launch saves only the round trip of t: the two unfused launches measure as fast (v8n c = 64 on H100)
+  // and the forward faster, so such a pair stays unfused.
+  if (plan->occ == 1 && !shortcut) {
+    delete plan;
+    return fail("one CTA per SM and no shortcut: the unfused pair is as fast");
+  }
+  plan->smem = (size_t)a.stages * a.slot + fixed + 1024;
+  dispatch_nt16(nm16, [&](auto m) {
+    dispatch_nt16(no16, [&](auto o) {
+      constexpr int M = decltype(m)::value, O = decltype(o)::value;
+      if constexpr (M <= BN_MAX_C / 16 && O <= BN_MAX_C / 16) plan->kernel = bneck_tc_kernel<M, O>;
+    });
+  });
+  cudaFuncSetAttribute(plan->kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  // plans of different shapes share an instantiation: its limit only ever grows to the largest plan made so far, so a
+  // smaller plan created later cannot make an earlier one's launch fail
+  static std::map<void (*)(BnArgs), size_t> smem_limit;
+  size_t& lim = smem_limit[plan->kernel];
+  if (plan->smem > lim) {
+    cudaError_t ce = cudaFuncSetAttribute(plan->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan->smem);
+    if (ce != cudaSuccess) {
+      delete plan;
+      return fail("cudaFuncSetAttribute(bneck_tc_kernel) failed");
+    }
+    lim = plan->smem;
+  }
+  int dev = 0, num_sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+  plan->grid = num_sms * plan->occ;
+  return plan;
+}
+
+std::string tc_bneck_plan_describe(const TcBneckPlan* plan) {
+  const BnArgs& a = plan->args;
+  char buf[256];
+  snprintf(buf, sizeof(buf), "fused bottleneck %d->%d BK %d/%d chunks %d/%d shortcut %d stages %d occ %d smem %zu KiB grid %d",
+           a.cmid, a.cout, a.BK1, a.BK2, a.chunks1, a.chunks2, a.shortcut, a.stages, plan->occ, plan->smem / 1024, plan->grid);
+  return buf;
+}
+
+void tc_bneck_plan_destroy(TcBneckPlan* plan) { delete plan; }  // the weight slabs belong to the two conv plans
+
+int tc_bneck_launch(const TcBneckPlan* plan, int B, int* tile_ctr, cudaStream_t s) {
+  BnArgs a = plan->args;
+  a.tiles_w = (a.W + HALO_BW - 1) / HALO_BW;
+  a.tiles_h = (a.H + HALO_BH - 1) / HALO_BH;
+  a.total_tiles = B * a.tiles_w * a.tiles_h;
+  auto magic = [](int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); };
+  a.m_tpi = magic(a.tiles_w * a.tiles_h); a.m_tw = magic(a.tiles_w);
+  a.tile_ctr = tile_ctr;
+  const int grid = std::min(plan->grid, a.total_tiles);
+  a.tile_batch = std::max(1, std::min(8, a.total_tiles / (4 * grid)));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(TC_THREADS);
+  cfg.dynamicSmemBytes = plan->smem;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;  // PDL (see griddepcontrol in the kernel)
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
   YB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, plan->kernel, a));
   return 0;
 }

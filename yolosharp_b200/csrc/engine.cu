@@ -73,6 +73,8 @@ struct OpDesc {
   int dep_op = -1;     // layer chaining: the op whose per-image completion gates this op's tiles (-1: whole previous grid)
   EpiDecode dec;       // conv: fused Detect-tail epilogue (tensor-core path)
   bool fused = false;  // decode op: its work is done by the producing convs' epilogues
+  TcBneckPlan* bneck = nullptr;  // conv: fused Bottleneck that also computes the previous op (its input) in smem
+  bool absorbed = false;         // conv: computed inside the next op's fused Bottleneck launch; launches nothing
 };
 
 struct HostTensor {
@@ -730,7 +732,10 @@ static int run_ops(yb_engine* e, const void* in, int in_dtype, int B, float* out
           if (rc) return rc;
           input_converted = true;
         }
-        if (op.use_tc) {
+        if (op.absorbed) break;
+        if (op.bneck) {
+          rc = tc_bneck_launch(op.bneck, B, e->tile_ctr ? e->tile_ctr + i : nullptr, s);
+        } else if (op.use_tc) {
           TcChain ch;
           const bool chained = e->chain != 0 && only < 0;
           if (chained) {
@@ -889,6 +894,7 @@ void yb_destroy(yb_engine* e) {
   if (e->cfg.flags & YB_FLAG_DRY_RUN) { delete e; return; }
   cudaSetDevice(e->cfg.device);
   for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
+  for (auto& op : e->ops) if (op.bneck) tc_bneck_plan_destroy(op.bneck);
   for (auto& op : e->ops) if (op.plan) tc_conv_plan_destroy(op.plan);
   for (void* p : e->dev_allocs) cudaFree(p);
   if (e->arena) cudaFree(e->arena);
@@ -1027,6 +1033,28 @@ int32_t yb_finalize_weights(yb_engine* e) {
         return YB_ERR_STATE;
       }
   }
+  // Bottleneck fusion: a 3x3 s1 tensor-core conv whose output buffer has exactly one reader, the next 3x3 s1 conv of the
+  // same lane, runs inside that conv's launch (tc_bneck_plan_create decides whether the pair fits).  The first op stays in
+  // the op list, launches nothing and keeps its arena buffer for yb_debug_read_activation.
+  for (size_t i = 1; i + 1 < e->ops.size(); i++) {
+    OpDesc &a = e->ops[i], &b = e->ops[i + 1];
+    if (a.type != OP_CONV || b.type != OP_CONV || !a.use_tc || !b.use_tc || a.absorbed || a.bneck) continue;
+    if (a.k != 3 || a.s != 1 || b.k != 3 || b.s != 1 || a.lane != b.lane) continue;
+    if (b.in.buf != a.out.buf || b.in.coff != a.out.coff || b.in.C != a.out.C) continue;
+    bool single = true;
+    for (size_t j = 0; j < e->ops.size(); j++) {
+      const OpDesc& o = e->ops[j];
+      if (j == i || j == i + 1) continue;
+      for (const VRef* r : {&o.in, &o.out, &o.res, &o.out2, &o.out3, &o.cls, &o.coef})
+        if (r->buf == a.out.buf) single = false;
+    }
+    if (!single || b.res.buf == a.out.buf) continue;
+    std::string err;
+    b.bneck = tc_bneck_plan_create(a.plan, b.plan, &err);
+    if (!b.bneck) continue;
+    a.absorbed = true;
+    if (getenv("YB_DEBUG_PLANS")) fprintf(stderr, "[plan] %-30s %s (absorbs %s)\n", b.name.c_str(), tc_bneck_plan_describe(b.bneck).c_str(), a.name.c_str());
+  }
   // Layer chaining: inside a lane, a tensor-core conv whose stream predecessor is a tensor-core conv that stores an NHWC
   // tensor starts its tiles per image, as soon as the predecessor has stored that image (per-image counters), instead
   // of waiting for the predecessor's whole grid.  Completion per image is monotone along the lane (every op waits for
@@ -1039,12 +1067,13 @@ int32_t yb_finalize_weights(yb_engine* e) {
     for (int l = 0; l < yb_engine::kLanes; l++) prev_in_lane[l] = -1;
     for (size_t i = 0; i < e->ops.size(); i++) {
       OpDesc& op = e->ops[i];
-      if (op.type == OP_DECODE && op.fused) continue;  // launches nothing
+      if ((op.type == OP_DECODE && op.fused) || op.absorbed) continue;  // launches nothing
       const int lane = (e->cfg.flags & YB_FLAG_NO_CONCURRENCY) ? 0 : op.lane;
       const int pv = prev_in_lane[lane];
-      if (op.type == OP_CONV && op.use_tc && pv >= 0) {
+      // fused Bottlenecks neither wait on nor publish per-image counters: they keep the grid-wide dependency both ways
+      if (op.type == OP_CONV && op.use_tc && !op.bneck && pv >= 0) {
         const OpDesc& pr = e->ops[pv];
-        if (pr.type == OP_CONV && pr.use_tc && pr.dec.mode == EPI_STORE) op.dep_op = pv;
+        if (pr.type == OP_CONV && pr.use_tc && !pr.bneck && pr.dec.mode == EPI_STORE) op.dep_op = pv;
       }
       prev_in_lane[lane] = (int)i;
     }
@@ -1398,9 +1427,17 @@ int32_t yb_debug_read_activation(yb_engine* e, int32_t op_index, int32_t batch, 
   chw[0] = v.C; chw[1] = v.H; chw[2] = v.W;
   const int64_t n = (int64_t)batch * v.C * v.H * v.W;
   if (n > host_capacity) { set_error("yb_debug_read_activation: host buffer too small"); return YB_ERR_INVALID_ARG; }
+  int rc = 0;
+  if (op.absorbed) {
+    // The fused Bottleneck kept this op's output in shared memory only: materialise it now into the op's own arena
+    // buffer with the fp16 CUDA-core twin (same fp16-rounded weights).  Its input slice is still what the last forward
+    // read, because arena buffers are never reused within a forward.
+    rc = launch_conv_generic<__half>(conv_params(e, op, batch), 0);
+    if (rc) return rc;
+  }
   float* d = nullptr;
   YB_CUDA_CHECK(cudaMalloc((void**)&d, n * sizeof(float)));
-  int rc = e->cfg.precision == YB_PREC_F16 ? launch_view_to_nchw_f32<__half>(v, d, batch, 0)
+  rc = e->cfg.precision == YB_PREC_F16 ? launch_view_to_nchw_f32<__half>(v, d, batch, 0)
                                            : launch_view_to_nchw_f32<float>(v, d, batch, 0);
   if (!rc && cudaMemcpy(host_out, d, n * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess) {
     set_error("yb_debug_read_activation: copy failed");
@@ -1478,6 +1515,11 @@ int32_t yb_op_cost(const yb_engine* e, int32_t i, int32_t batch, double* flops, 
       *bytes -= vbytes(op.in);
       *bytes += (double)batch * 3 * e->cfg.height * e->cfg.width * e->esize;
     }
+    if (op.absorbed) *bytes = 0;  // moved by the fused Bottleneck launch of the next op
+    if (op.bneck) {               // reads the block input (once, also as the shortcut) and both weight sets
+      const OpDesc& pa = e->ops[i - 1];
+      *bytes = vbytes(pa.in) + vbytes(op.out) + (double)(pa.cout * pa.cin + op.cout * op.cin) * 9 * e->esize;
+    }
   } else if (op.type == OP_DECODE) {
     *bytes = vbytes(op.in) + vbytes(op.cls) + vbytes(op.coef) +
              (double)batch * e->pred_c * e->bufs[op.in.buf].H * e->bufs[op.in.buf].W * 4.0;
@@ -1510,7 +1552,7 @@ int32_t yb_launches_per_forward(const yb_engine* e) {
   if (!e) return 0;
   int n = e->has_stem_tc ? 0 : 1;  // generic path converts the input layout first
   for (const OpDesc& op : e->ops)
-    if (!(op.type == OP_DECODE && op.fused)) n++;
+    if (!(op.type == OP_DECODE && op.fused) && !op.absorbed) n++;
   return n;
 }
 
