@@ -475,6 +475,36 @@ int32_t yb_op_cost(const yb_engine* e, int32_t op_index, int32_t batch, double* 
 int32_t yb_op_kind(const yb_engine* e, int32_t op_index);
 /* debug: the `skip`-th tensor-core conv launch from now records a clock64 timeline of CTA 0 into dev_buf (128 x int64) */
 int32_t yb_debug_timeline(long long* dev_buf, int32_t skip);
+/* debug: ONE launch of the fp16 tensor-core convolution (conv_tc_kernel) on caller-owned device buffers, planned as the
+ * engine plans its layers; synchronises before it returns.  Op-level tests compare it with a float64 convolution.
+ *   in      fp16 NHWC (plan_batch, height, width, in_pitch), the input channels at [in_coff, in_coff + cin)
+ *   w       fp16 [cout][k][k][cin];  bias float32 (cout);  k 1 (stride 1) or 3 (stride 1 or 2), pad k / 2;  act 0 / 1 (SiLU)
+ *   res     fp16 (plan_batch, Ho, Wo, res_pitch) added after the activation at [res_coff, ..), or NULL
+ *   out     fp16 (plan_batch, Ho, Wo, out_pitch), written at [out_coff, out_coff + cout); NULL with a decode epilogue
+ *   plan_batch / run_batch  images the plan is made for / launched with (run_batch <= plan_batch)
+ *   share_sms   1: the grid trimming of a layer that shares the GPU with a sibling head branch
+ *   tile_counter  1: dynamic tile queue, 0: static round-robin tile order
+ *   dec_*   fused Detect epilogue of a 1x1 conv (dec_mode 1 DFL box, 2 sigmoid, 3 raw; 0 = store into out): pred float32
+ *           (run_batch, dec_channels, dec_anchors) receives anchors dec_a0 .. dec_a0 + dec_pixels - 1 of a level dec_width
+ *           pixels wide, channels dec_ch0 .. (rows 0-3 for the box), box coordinates times dec_stride
+ *   desc    receives the plan description (tc_conv_plan_describe), or NULL
+ * A shape the tensor-core conv or its planner does not take returns YB_ERR_SHAPE with the reason. */
+int32_t yb_debug_conv_f16(const void* in, int32_t plan_batch, int32_t run_batch, int32_t height, int32_t width, int32_t in_pitch,
+                          int32_t in_coff, int32_t cin, const void* w, const float* bias, int32_t cout, int32_t k, int32_t stride,
+                          int32_t act, const void* res, int32_t res_pitch, int32_t res_coff, void* out, int32_t out_pitch,
+                          int32_t out_coff, int32_t share_sms, int32_t tile_counter, int32_t dec_mode, int32_t dec_anchors,
+                          int32_t dec_channels, int32_t dec_a0, int32_t dec_ch0, int32_t dec_width, int32_t dec_pixels,
+                          float dec_stride, float* pred, char* desc, int32_t desc_capacity);
+/* debug: ONE launch of the fused Bottleneck kernel (bneck_tc_kernel) on caller-owned device buffers: out = SiLU(conv_b(t) +
+ * bias_b) [+ x], t = fp16(SiLU(conv_a(x) + bias_a)), both 3x3 stride 1; synchronises before it returns.
+ *   x       fp16 NHWC (batch, height, width, x_pitch), channels [x_coff, x_coff + cin); also the shortcut when shortcut != 0
+ *   w_a     fp16 [cmid][3][3][cin], bias_a float32 (cmid);  w_b fp16 [cout][3][3][cmid], bias_b float32 (cout)
+ *   out     fp16 (batch, height, width, out_pitch), written at [out_coff, out_coff + cout)
+ *   desc    receives the fused plan's description (tc_bneck_plan_describe), or NULL
+ * A pair the fused kernel does not take returns YB_ERR_SHAPE with the planner's reason. */
+int32_t yb_debug_bneck_f16(const void* x, int32_t batch, int32_t height, int32_t width, int32_t x_pitch, int32_t x_coff, int32_t cin,
+                           const void* w_a, const float* bias_a, int32_t cmid, const void* w_b, const float* bias_b, int32_t cout,
+                           int32_t shortcut, void* out, int32_t out_pitch, int32_t out_coff, char* desc, int32_t desc_capacity);
 
 #ifdef __cplusplus
 }

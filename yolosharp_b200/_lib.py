@@ -118,6 +118,11 @@ SIGNATURES = {
     "yb_op_cost": (c_i32, [c_vp, c_i32, c_i32, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "yb_op_kind": (c_i32, [c_vp, c_i32]),
     "yb_debug_timeline": (c_i32, [c_vp, c_i32]),
+    "yb_debug_conv_f16": (c_i32, [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32,
+                                  c_vp, c_i32, c_i32, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32,
+                                  c_i32, c_f32, c_vp, c_vp, c_i32]),
+    "yb_debug_bneck_f16": (c_i32, [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_i32, c_vp,
+                                   c_i32, c_i32, c_vp, c_i32]),
 }
 
 _lib = None

@@ -1535,6 +1535,123 @@ int32_t yb_debug_timeline(long long* dev_buf, int32_t skip) {
   return YB_OK;
 }
 
+static void copy_desc(const std::string& s, char* desc, int32_t cap) {
+  if (desc && cap > 0) snprintf(desc, (size_t)cap, "%s", s.c_str());
+}
+
+// Launches a tensor-core plan (fused Bottleneck when `bn` is set) with a zeroed tile counter (or none) on the legacy
+// stream and waits for it.
+static int run_debug_launch(const TcConvPlan* plan, const TcBneckPlan* bn, int B, float* pred, bool tile_counter,
+                            const char* who) {
+  int* ctr = nullptr;
+  if (tile_counter) {
+    YB_CUDA_CHECK(cudaMalloc((void**)&ctr, sizeof(int)));
+    YB_CUDA_CHECK(cudaMemset(ctr, 0, sizeof(int)));
+  }
+  int rc = bn ? tc_bneck_launch(bn, B, ctr, 0) : tc_conv_launch(plan, B, pred, ctr, 0);
+  const cudaError_t ce = cudaDeviceSynchronize();
+  if (!rc && ce != cudaSuccess) {
+    set_error(std::string(who) + ": kernel failed: " + cudaGetErrorString(ce));
+    rc = YB_ERR_CUDA;
+  }
+  if (ctr) cudaFree(ctr);
+  return rc;
+}
+
+int32_t yb_debug_conv_f16(const void* in, int32_t plan_batch, int32_t run_batch, int32_t height, int32_t width, int32_t in_pitch,
+                          int32_t in_coff, int32_t cin, const void* w, const float* bias, int32_t cout, int32_t k, int32_t stride,
+                          int32_t act, const void* res, int32_t res_pitch, int32_t res_coff, void* out, int32_t out_pitch,
+                          int32_t out_coff, int32_t share_sms, int32_t tile_counter, int32_t dec_mode, int32_t dec_anchors,
+                          int32_t dec_channels, int32_t dec_a0, int32_t dec_ch0, int32_t dec_width, int32_t dec_pixels,
+                          float dec_stride, float* pred, char* desc, int32_t desc_capacity) {
+  const bool decode = dec_mode != EPI_STORE;
+  if (!in || !w || !bias || (decode ? !pred : !out)) { set_error("yb_debug_conv_f16: null argument"); return YB_ERR_INVALID_ARG; }
+  if (plan_batch <= 0 || run_batch <= 0 || run_batch > plan_batch || height <= 0 || width <= 0 || cin <= 0 || cout <= 0 ||
+      in_coff < 0 || in_pitch < in_coff + cin || (k != 1 && k != 3) || stride <= 0 || (act != ACT_NONE && act != ACT_SILU) ||
+      dec_mode < EPI_STORE || dec_mode > EPI_RAW || (!decode && (out_coff < 0 || out_pitch < out_coff + cout)) ||
+      (res && (res_coff < 0 || res_pitch < res_coff + cout))) {
+    set_error("yb_debug_conv_f16: bad argument (batch, extent, channel view, k, stride, act or decode mode)");
+    return YB_ERR_INVALID_ARG;
+  }
+  ConvParams p;
+  p.B = plan_batch;
+  p.Cin = cin; p.Cout = cout;
+  p.k = k; p.stride = stride; p.pad = k / 2;
+  p.Ho = (height + 2 * p.pad - k) / stride + 1;
+  p.Wo = (width + 2 * p.pad - k) / stride + 1;
+  p.act = act;
+  p.w = w; p.bias = bias;
+  p.share_sms = share_sms ? 1 : 0;
+  p.in.base = const_cast<void*>(in); p.in.H = height; p.in.W = width; p.in.pitch = in_pitch; p.in.coff = in_coff; p.in.C = cin;
+  p.out.base = out; p.out.H = p.Ho; p.out.W = p.Wo; p.out.pitch = out_pitch; p.out.coff = out_coff; p.out.C = cout;
+  if (res) {
+    p.res.base = const_cast<void*>(res); p.res.H = p.Ho; p.res.W = p.Wo; p.res.pitch = res_pitch; p.res.coff = res_coff; p.res.C = cout;
+  }
+  p.dec.mode = dec_mode; p.dec.A = dec_anchors; p.dec.Ctot = dec_channels; p.dec.a0 = dec_a0; p.dec.ch0 = dec_ch0;
+  p.dec.Wl = dec_width; p.dec.HW = dec_pixels; p.dec.stride = dec_stride;
+  if (!tc_conv_supported(p)) {
+    set_error("yb_debug_conv_f16: shape not supported by the tensor-core conv (Cin, Cout % 16, Cout <= 1024, k / stride, "
+              "channel offsets and pitches % 8)");
+    return YB_ERR_SHAPE;
+  }
+  if (!have_device("yb_debug_conv_f16")) return YB_ERR_NO_DEVICE;
+  std::string err;
+  TcConvPlan* plan = tc_conv_plan_create(p, &err);
+  if (!plan) { set_error("yb_debug_conv_f16: " + err); return YB_ERR_SHAPE; }
+  copy_desc(tc_conv_plan_describe(plan), desc, desc_capacity);
+  const int rc = run_debug_launch(plan, nullptr, run_batch, pred, tile_counter != 0, "yb_debug_conv_f16");
+  tc_conv_plan_destroy(plan);
+  return rc;
+}
+
+int32_t yb_debug_bneck_f16(const void* x, int32_t batch, int32_t height, int32_t width, int32_t x_pitch, int32_t x_coff, int32_t cin,
+                           const void* w_a, const float* bias_a, int32_t cmid, const void* w_b, const float* bias_b, int32_t cout,
+                           int32_t shortcut, void* out, int32_t out_pitch, int32_t out_coff, char* desc, int32_t desc_capacity) {
+  if (!x || !w_a || !bias_a || !w_b || !bias_b || !out) { set_error("yb_debug_bneck_f16: null argument"); return YB_ERR_INVALID_ARG; }
+  if (batch <= 0 || height <= 0 || width <= 0 || cin <= 0 || cmid <= 0 || cout <= 0 || x_coff < 0 || x_pitch < x_coff + cin ||
+      out_coff < 0 || out_pitch < out_coff + cout) {
+    set_error("yb_debug_bneck_f16: bad argument (batch, extent or channel view)");
+    return YB_ERR_INVALID_ARG;
+  }
+  // conv a writes t into a dense scratch buffer (the fused kernel never touches it: it only needs the plan), conv b reads it
+  ConvParams pa;
+  pa.B = batch; pa.Cin = cin; pa.Cout = cmid;
+  pa.k = 3; pa.stride = 1; pa.pad = 1; pa.Ho = height; pa.Wo = width;
+  pa.act = ACT_SILU; pa.w = w_a; pa.bias = bias_a;
+  pa.in.base = const_cast<void*>(x); pa.in.H = height; pa.in.W = width; pa.in.pitch = x_pitch; pa.in.coff = x_coff; pa.in.C = cin;
+  pa.out.H = height; pa.out.W = width; pa.out.pitch = cmid; pa.out.coff = 0; pa.out.C = cmid;
+  ConvParams pb = pa;
+  pb.Cin = cmid; pb.Cout = cout; pb.w = w_b; pb.bias = bias_b;
+  pb.in = pa.out;
+  pb.out.base = out; pb.out.pitch = out_pitch; pb.out.coff = out_coff; pb.out.C = cout;
+  if (shortcut) pb.res = pa.in;
+  if (!tc_conv_supported(pa) || !tc_conv_supported(pb)) {
+    set_error("yb_debug_bneck_f16: shape not supported by the tensor-core conv (channels % 16, channel offsets and pitches % 8)");
+    return YB_ERR_SHAPE;
+  }
+  if (!have_device("yb_debug_bneck_f16")) return YB_ERR_NO_DEVICE;
+  void* t = nullptr;
+  YB_CUDA_CHECK(cudaMalloc(&t, (size_t)batch * height * width * cmid * sizeof(__half)));
+  pa.out.base = pb.in.base = t;
+  std::string err;
+  TcConvPlan* plan_a = tc_conv_plan_create(pa, &err);
+  TcConvPlan* plan_b = plan_a ? tc_conv_plan_create(pb, &err) : nullptr;
+  TcBneckPlan* bn = plan_b ? tc_bneck_plan_create(plan_a, plan_b, &err) : nullptr;
+  int rc = 0;
+  if (!bn) {
+    set_error("yb_debug_bneck_f16: " + err);
+    rc = YB_ERR_SHAPE;
+  } else {
+    copy_desc(tc_bneck_plan_describe(bn), desc, desc_capacity);
+    rc = run_debug_launch(nullptr, bn, batch, nullptr, true, "yb_debug_bneck_f16");
+  }
+  tc_bneck_plan_destroy(bn);
+  tc_conv_plan_destroy(plan_b);
+  tc_conv_plan_destroy(plan_a);
+  cudaFree(t);
+  return rc;
+}
+
 int32_t yb_op_kind(const yb_engine* e, int32_t i) {
   if (!e || i < 0 || i >= (int32_t)e->ops.size()) return -1;
   const OpDesc& op = e->ops[i];

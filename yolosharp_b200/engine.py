@@ -481,6 +481,60 @@ def conv_forward_tc(x, w, bias=None, stride=1, pad=None, ws=None, stream=None):
     return z
 
 
+def _ptr(t):
+    return C.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _f16_nhwc(t):
+    assert t.is_cuda and t.dtype == torch.float16 and t.is_contiguous() and t.dim() == 4
+    return t
+
+
+def debug_conv_f16(x, w, bias, out=None, stride=1, act=1, x_coff=0, out_coff=0, res=None, res_coff=0, plan_batch=None,
+                   run_batch=None, share_sms=False, tile_counter=True, decode=None, pred=None):
+    """yb_debug_conv_f16: one launch of the fp16 tensor-core conv on caller buffers -> the plan description.
+    x (B, H, W, pitch) fp16 with the input at channels [x_coff, x_coff + Cin); w (Cout, k, k, Cin) fp16; bias (Cout) fp32;
+    out / res (B, Ho, Wo, pitch) fp16 written / read at [out_coff, ..) / [res_coff, ..); plan_batch defaults to B, run_batch
+    to plan_batch.  decode = dict(mode, A, Ctot, a0, ch0, Wl, HW, stride) writes pred (run_batch, Ctot, A) fp32 instead."""
+    _f16_nhwc(x)
+    assert w.is_cuda and w.dtype == torch.float16 and w.is_contiguous() and w.dim() == 4 and w.shape[1] == w.shape[2]
+    assert bias.is_cuda and bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == w.shape[0]
+    for t in (out, res):
+        if t is not None:
+            _f16_nhwc(t)
+    B, H, W, pitch = x.shape
+    Cout, k, _, Cin = w.shape
+    plan_batch = plan_batch or B
+    run_batch = run_batch or plan_batch
+    d = decode or {}
+    if decode is not None:
+        assert pred is not None and pred.is_cuda and pred.dtype == torch.float32 and pred.is_contiguous()
+    desc = C.create_string_buffer(256)
+    L.check(L.lib().yb_debug_conv_f16(
+        _ptr(x), plan_batch, run_batch, H, W, pitch, x_coff, Cin, _ptr(w), _ptr(bias), Cout, k, stride, int(act),
+        _ptr(res), res.shape[3] if res is not None else 0, res_coff, _ptr(out), out.shape[3] if out is not None else 0, out_coff,
+        int(share_sms), int(tile_counter), d.get("mode", 0), d.get("A", 0), d.get("Ctot", 0), d.get("a0", 0), d.get("ch0", 0),
+        d.get("Wl", 0), d.get("HW", 0), float(d.get("stride", 0.0)), _ptr(pred), desc, len(desc)))
+    return desc.value.decode()
+
+
+def debug_bneck_f16(x, w_a, bias_a, w_b, bias_b, out, shortcut=True, x_coff=0, out_coff=0):
+    """yb_debug_bneck_f16: one launch of the fused Bottleneck kernel -> the fused plan's description.
+    x (B, H, W, pitch) fp16 with the block input at [x_coff, x_coff + cin); w_a (cmid, 3, 3, cin), w_b (cout, 3, 3, cmid) fp16;
+    biases fp32; out (B, H, W, pitch) fp16 written at [out_coff, out_coff + cout)."""
+    _f16_nhwc(x)
+    _f16_nhwc(out)
+    for w, b in ((w_a, bias_a), (w_b, bias_b)):
+        assert w.is_cuda and w.dtype == torch.float16 and w.is_contiguous() and tuple(w.shape[1:3]) == (3, 3)
+        assert b.is_cuda and b.dtype == torch.float32 and b.is_contiguous() and b.numel() == w.shape[0]
+    B, H, W, pitch = x.shape
+    desc = C.create_string_buffer(256)
+    L.check(L.lib().yb_debug_bneck_f16(_ptr(x), B, H, W, pitch, x_coff, w_a.shape[3], _ptr(w_a), _ptr(bias_a), w_a.shape[0],
+                                       _ptr(w_b), _ptr(bias_b), w_b.shape[0], int(shortcut), _ptr(out), out.shape[3], out_coff,
+                                       desc, len(desc)))
+    return desc.value.decode()
+
+
 def conv_backward_tc(x, dz, w, stride=1, pad=None, ws=None, stream=None, need_dx=True):
     """yb_conv_backward_data_tc / _weight_tc -> (dx, dw); same tensors as conv_backward."""
     for t in (x, dz, w):
