@@ -469,9 +469,14 @@ int32_t yb_profile_forward(yb_engine* e, const void* in, int32_t in_dtype, int32
 int32_t yb_time_op(yb_engine* e, int32_t op_index, const void* in, int32_t in_dtype, int32_t batch, float* out_pred,
                    float* out_proto, int32_t reps, float* ms_per_launch, void* stream);
 /* Algorithmic work of op i for `batch` images: flops = 2*MACs (convs only), bytes = input view +
- * output view (+ residual) + weights, each counted once (SURVEY.md section 8(d) definitions). */
+ * output view (+ residual) + weights, each counted once (SURVEY.md section 8(d) definitions).  An op fused into the
+ * next op's launch reports the bytes of that launch there: the first conv of a fused Bottleneck keeps its FLOPs and
+ * reports 0 bytes; a conv folded into a 1x1 reports 0 FLOPs and 0 bytes, and the 1x1 reports both convs' FLOPs and
+ * the producer's input, both weight sets and its own output. */
 int32_t yb_op_cost(const yb_engine* e, int32_t op_index, int32_t batch, double* flops, double* bytes);
-/* 0 = tensor-core conv, 1 = CUDA-core conv, 2 = stem, 3 = depthwise, 4 = pool, 5 = upsample, 6 = decode, 7 = other */
+/* 0 = tensor-core conv, 1 = CUDA-core conv, 2 = stem, 3 = depthwise, 4 = pool, 5 = upsample, 7 = other;
+ * 6 = launches nothing of its own and reports no FLOPs or bytes: a fused Detect decode, or a conv folded into the next
+ * op's 1x1 launch (that op reports the FLOPs of both convs and the bytes its launch moves) */
 int32_t yb_op_kind(const yb_engine* e, int32_t op_index);
 /* debug: the `skip`-th tensor-core conv launch from now records a clock64 timeline of CTA 0 into dev_buf (128 x int64) */
 int32_t yb_debug_timeline(long long* dev_buf, int32_t skip);

@@ -168,6 +168,11 @@ TcBneckPlan* tc_bneck_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, st
 void tc_bneck_plan_destroy(TcBneckPlan* plan);
 std::string tc_bneck_plan_describe(const TcBneckPlan* plan);
 int tc_bneck_launch(const TcBneckPlan* plan, int B, int* tile_ctr, cudaStream_t s);
+// Folded 1x1 (DESIGN 4.1): the conv `pa` and the 1x1 conv `pb` that is the only reader of its output as one
+// conv_tc_kernel launch; `pa`'s activations go from its accumulator to `pb`'s MMA in registers and are never stored.
+// The result is an ordinary plan (tc_conv_launch / describe / destroy) that uses both plans' packed weights, so they
+// must outlive it.  nullptr (and the reason in *err) when the pair does not fit.
+TcConvPlan* tc_fold_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, std::string* err);
 // stem: NCHW u8/f16/f32 input -> 3x3 s2 conv (Cin=3) + bias + SiLU -> NHWC fp16
 int launch_stem_f16(const void* in, int in_dtype, int B, int H, int W, const __half* w16 /*[Cout][32]*/,
                     const float* bias, const View& out, cudaStream_t s, int src_H = 0, int src_W = 0);  // src_*: unpadded source size

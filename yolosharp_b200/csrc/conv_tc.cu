@@ -78,6 +78,12 @@ struct TcArgs {
   int* tile_ctr;   // dynamic tile scheduler: global counter of this launch (nullptr = static round-robin)
   int tile_batch;  // consecutive tiles drawn per atomicAdd (one counter address serves the whole grid)
   long long* dbg;  // optional timeline buffer (tools/exp_timeline.py); nullptr in production
+  // folded 1x1 (tc_fold, conv_tc_kernel<NT16, N2_16 > 0>): this conv's activations never leave registers; the next conv, a
+  // 1x1, multiplies them with its weights and runs the epilogue described above (out / act / epi_mode are the 1x1's)
+  const uint8_t* w2;  // the 1x1's packed weight slabs (pack_weights_kernel, taps = 1), resident in smem at w2_off
+  const float* bias2;
+  uint32_t w2_off, w2_bytes, b2_stride, sbo_b2, layout_b2;
+  int BK2, n2, act1;  // the 1x1's slab width and Cout; this conv's activation
 };
 
 struct TcConvPlan {
@@ -89,7 +95,8 @@ struct TcConvPlan {
   size_t smem;
   int grid;
   uint8_t* wpk = nullptr;  // device, owned: packed weight slabs
-  void (*kernel)(TcArgs) = nullptr;  // conv_tc_kernel<n_tile / 16>
+  void (*kernel)(TcArgs) = nullptr;  // conv_tc_kernel<n_tile / 16> (<n_tile / 16, fold16> for a folded 1x1)
+  int fold16 = 0;                    // folded 1x1 (tc_fold_plan_create): its column pass width / 16
 };
 
 __device__ __forceinline__ int fdiv(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
@@ -101,6 +108,11 @@ __device__ __forceinline__ float silu_tanh(float v) {
   float t;
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));
   return fmaf(h, t, h);
+}
+
+__device__ __forceinline__ uint32_t pack_h2(float x, float y) {
+  const __half2 h = __floats2half2_rn(x, y);
+  return *reinterpret_cast<const uint32_t*>(&h);
 }
 
 constexpr int TC_CONSUMERS = 256;                // warps 0-7: two warpgroups, rows 0-63 / 64-127 of every tile
@@ -299,24 +311,27 @@ __device__ __forceinline__ void tc_epilogue(const TcArgs& a, const float* acc, c
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t4 = lane & 3;
   size_t pix[2];
+  int ho[2];
 #pragma unroll
   for (int h = 0; h < 2; h++) {
     const int row = wg * 64 + (warp & 3) * 16 + g + 8 * h;
     const int hl = fdiv(row, a.m_bw), wl = row - hl * a.BW;
-    const int ho = th * a.BH + hl;
+    ho[h] = th * a.BH + hl;
     wo[h] = tw * a.BW + wl;
-    valid[h] = hl < a.BH && ho < a.Ho && wo[h] < a.Wo;
-    pix[h] = ((size_t)img * a.Ho + ho) * a.Wo + wo[h];
+    valid[h] = hl < a.BH && ho[h] < a.Ho && wo[h] < a.Wo;
+    pix[h] = ((size_t)img * a.Ho + ho[h]) * a.Wo + wo[h];
   }
   if (a.epi_mode != EPI_STORE) {
-    // fused Detect tail (flattened 1x1 conv): row h of this thread is pixel wo[h] of the whole batch
+    // fused Detect tail: row h of this thread is anchor i of image n - pixel wo[h] of the whole batch for a flattened
+    // tile, (ho, wo) of image img for a rectangular one (a 1x1 folded into a 3x3 producer)
+    const bool flat1 = a.imgs == 1 && a.Ho == 1;
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-      const int n = valid[h] ? wo[h] / a.dHW : 0;
-      const int i = wo[h] - n * a.dHW;
+      const int n = flat1 ? (valid[h] ? wo[h] / a.dHW : 0) : img;
+      const int i = flat1 ? wo[h] - n * a.dHW : ho[h] * a.dWl + wo[h];
       float* po = a.pred + (size_t)n * a.dCtot * a.dA + a.da0 + i;
       if (a.epi_mode == EPI_DFL_BOX) {
-        if constexpr (NT16 == 4) {  // tc_conv_plan_create refuses a DFL plan whose n_tile is not 64 = 4 sides x 16 bins
+        if constexpr (NT16 == 4) {  // the plans refuse a DFL epilogue whose n_tile / pass is not 64 = 4 sides x 16 bins
           // DFL (Block.cs:44): softmax over the 16 bins of each side, expectation with weights 0..15; then
           // dist2bbox(xywh) * stride (Tal.cs:338-356, Head.cs:221).  A quad of lanes holds the 16 bins of a side.
           float d[4];
@@ -359,7 +374,7 @@ __device__ __forceinline__ void tc_epilogue(const TcArgs& a, const float* acc, c
             const int c = 8 * J + 2 * t4 + e;
             float f = acc[4 * J + 2 * h + e] + bias[c];
             if (a.epi_mode == EPI_SIGMOID) f = __fdividef(1.0f, 1.0f + __expf(-f));
-            po[(size_t)(a.dch0 + c) * a.dA] = f;
+            po[(size_t)(a.dch0 + n0 + c) * a.dA] = f;
           }
       }
     }
@@ -389,8 +404,64 @@ __device__ __forceinline__ void tc_epilogue(const TcArgs& a, const float* acc, c
   }
 }
 
-template <int NT16>
-__global__ void __launch_bounds__(TC_THREADS, NT16 <= 4 ? 2 : 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
+// Folded 1x1 of one tile for one consumer warpgroup.  The tile's accumulator (this conv, NT16 * 16 channels) goes
+// through the unfused store path's +bias -> activation -> fp16 rounding, but into registers: f16 pairs in the A-fragment
+// layout, 16 channels per k16 step (tc_ptx.cuh, wgmma_f16_rs).  The 1x1 then runs in passes of F16 * 16 output
+// columns against its resident weight slabs, each pass followed by the 1x1's epilogue.  Its k16 steps are those of the
+// unfused 1x1 launch, in the same channel order on the same fp16 operands; that launch's extra steps over a ragged
+// last slab multiply zeros.  The passes are unrolled, so the fragments die with the last pass's MMAs, before its epilogue.
+__host__ __device__ constexpr int tc_fold_pass16(int n2_16) {  // column pass width / 16 (0: no pass width fits)
+  return n2_16 <= 5 ? n2_16 : (n2_16 % 4 == 0 ? 4 : (n2_16 % 5 == 0 ? 5 : 0));
+}
+
+template <int NT16, int N2_16, int KK2>
+__device__ __forceinline__ void tc_fold(const TcArgs& a, const float* acc, const float* bias1, const float* bias2,
+                                        uint32_t smemW2, int img, int th, int tw, int wg) {
+  constexpr int F16 = tc_fold_pass16(N2_16);
+  static_assert(F16 > 0 && N2_16 % F16 == 0, "the 1x1's Cout must split into column passes of <= 80");
+  const int t4 = threadIdx.x & 3;
+  uint32_t fr[NT16 * 4];
+#pragma unroll
+  for (int J = 0; J < NT16 * 2; J++) {
+    const int c = 8 * J + 2 * t4;
+    const float2 b = *reinterpret_cast<const float2*>(bias1 + c);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      float f0 = acc[4 * J + 2 * h] + b.x, f1 = acc[4 * J + 2 * h + 1] + b.y;
+      if (a.act1 == ACT_SILU) { f0 = silu_tanh(f0); f1 = silu_tanh(f1); }
+      fr[2 * J + h] = pack_h2(f0, f1);  // k step J / 2: fr[4 (J / 2) + 2 (J % 2) + h]
+    }
+  }
+  constexpr uint32_t ROW16 = KK2 * 2;  // bytes per weight row / 16
+  const uint32_t b_hi = wg_desc_hi(a.sbo_b2, a.layout_b2);
+  const uint32_t b_lo0 = wg_desc_lo(smemW2), b_slab16 = a.b2_stride >> 4;
+  bool valid[2];
+  int wo[2];
+#pragma unroll
+  for (int c0 = 0; c0 < 16 * N2_16; c0 += 16 * F16) {
+    float acc2[F16 * 8];
+    wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < NT16; kk++)
+      wg_mma_rs_n<F16>(acc2, fr + 4 * kk, b_lo0 + (kk / KK2) * b_slab16 + (uint32_t)c0 * ROW16 + 2 * (kk % KK2), b_hi, ROW16,
+                       kk > 0 ? 1u : 0u);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc<F16 * 8>(acc2);
+    tc_epilogue<F16>(a, acc2, bias2 + c0, c0, img, th, tw, wg, valid, wo);
+  }
+}
+
+constexpr int TC_FOLD_BIAS = 256;  // s_bias offset of the folded 1x1's bias (this conv has one N tile of <= 256)
+
+// CTAs per SM an instantiation's register bound allows without spills (ptxas -v): two leave 96 registers per thread,
+// room for 64 accumulator columns, or a fold whose two accumulators add up to that (32 -> 32).  A 64 -> 64 fold wants
+// ~150 registers and runs one CTA per SM.
+__host__ __device__ constexpr int tc_ctas_per_sm(int nt16, int n2_16) { return nt16 <= 4 && nt16 + n2_16 <= 4 ? 2 : 1; }
+
+// N2_16 > 0: a folded 1x1 of N2_16 * 16 output channels (tc_fold)
+template <int NT16, int N2_16 = 0>
+__global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_tc_kernel(const __grid_constant__ TcArgs a) {
   extern __shared__ __align__(1024) uint8_t tc_smem[];
   __shared__ __align__(8) uint64_t bars[4 * TC_MAX_STAGES + 1];
   __shared__ int s_tile[TQ];
@@ -399,6 +470,8 @@ __global__ void __launch_bounds__(TC_THREADS, NT16 <= 4 ? 2 : 1) conv_tc_kernel(
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int i = threadIdx.x; i < a.n_tile * a.n_tiles; i += blockDim.x) s_bias[i] = a.bias[i];  // constant data
+  if constexpr (N2_16 > 0)
+    for (int i = threadIdx.x; i < a.n2; i += blockDim.x) s_bias[TC_FOLD_BIAS + i] = a.bias2[i];
   // dynamic smem base rounded up to 1 KiB (SWIZZLE_128B atoms need it)
   const uint32_t smem0 = (smem_u32(tc_smem) + 1023u) & ~1023u;
   const uint32_t smemA = smem0;
@@ -434,11 +507,13 @@ __global__ void __launch_bounds__(TC_THREADS, NT16 <= 4 ? 2 : 1) conv_tc_kernel(
 
   if (warp == TC_CONSUMER_WARPS && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmA) : "memory");
-    if (a.b_resident) {
+    if (a.b_resident || N2_16 > 0) {
       // weights do not depend on the previous kernel: fetch them before the grid dependency resolves
-      mbar_arrive_expect_tx(bfull, a.b_bytes * a.ksteps);
-      for (int ks = 0; ks < a.ksteps; ks++)
-        bulk_load_1d(smemB + ks * a.b_stride, a.wpk + (size_t)ks * a.b_stride, a.b_bytes, bfull);
+      mbar_arrive_expect_tx(bfull, (a.b_resident ? a.b_bytes * a.ksteps : 0u) + (N2_16 > 0 ? a.w2_bytes : 0u));
+      if (a.b_resident)
+        for (int ks = 0; ks < a.ksteps; ks++)
+          bulk_load_1d(smemB + ks * a.b_stride, a.wpk + (size_t)ks * a.b_stride, a.b_bytes, bfull);
+      if (N2_16 > 0) bulk_load_1d(smem0 + a.w2_off, a.w2, a.w2_bytes, bfull);  // the folded 1x1's slabs, one copy
     }
   }
   // activations written by the previous kernel are visible only after this point - unless this launch is chained to
@@ -520,7 +595,7 @@ __global__ void __launch_bounds__(TC_THREADS, NT16 <= 4 ? 2 : 1) conv_tc_kernel(
     const int wg = warp >> 2;
     int sa = 0, sb = 0;
     uint32_t pa = 0, pb = 0;
-    if (a.b_resident) mbar_wait(bfull, 0);
+    if (a.b_resident || N2_16 > 0) mbar_wait(bfull, 0);
     int pend_img = -1, pend_cnt = 0;  // layer chaining: rows stored but not yet published
     const bool dbg_on = a.dbg && blockIdx.x == 0 && threadIdx.x == 0;
     for (int li = 0;; li++) {
@@ -540,6 +615,15 @@ __global__ void __launch_bounds__(TC_THREADS, NT16 <= 4 ? 2 : 1) conv_tc_kernel(
       const int r = mt - img * tiles_per_img;
       const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
       const int n0 = nt * a.n_tile;
+      if constexpr (N2_16 > 0) {  // one N tile: n0 = 0; never chained
+        switch (a.BK2) {
+          case 64: tc_fold<NT16, N2_16, 4>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, img, th, tw, wg); break;
+          case 32: tc_fold<NT16, N2_16, 2>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, img, th, tw, wg); break;
+          default: tc_fold<NT16, N2_16, 1>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, img, th, tw, wg); break;
+        }
+        if (dbg_on && li < 16) a.dbg[li * 8 + 6] = clock64();
+        continue;
+      }
       bool valid[2];
       int wo[2];
       tc_epilogue<NT16>(a, acc, s_bias + n0, n0, img, th, tw, wg, valid, wo);
@@ -620,6 +704,68 @@ static int pick_n_tile(int cout) {
   for (int n = 16; n <= cap; n += 16)
     if (cout % n == 0) best = n;
   return best;
+}
+
+static int tc_num_sms() {
+  static int num_sms = 0;
+  if (!num_sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return num_sms;
+}
+
+// Operand rings of a plan: stages, resident weights, CTAs per SM and dynamic shared memory.  `extra` bytes of the budget
+// hold the resident weights of a folded 1x1 (tc_fold_plan_create), placed after the rings at args.w2_off.  Returns
+// false when the tile does not fit.
+// Two CTAs per SM (each <= ~100 KiB smem) double the tiles in flight per SM and hide the producer -> MMA ->
+// epilogue hand-off latencies of the HBM-bound high-resolution layers; they need n_tile <= 64 (the register budget of
+// two 288-thread CTAs leaves room for 32 accumulator registers per thread).  Layers whose resident weights or wide N
+// tiles do not fit run one CTA per SM with the full budget.
+static bool tc_size_rings(TcConvPlan* plan, size_t extra, int max_occ) {
+  TcArgs& a = plan->args;
+  const ConvParams& p = plan->p;
+  const int num_sms = tc_num_sms();
+  const size_t b_all = (size_t)a.ksteps * a.b_stride;
+  const int m_tiles = plan->flat ? (p.B * p.Ho * p.Wo + 127) / 128
+                                 : p.B * ((p.Wo + a.BW - 1) / a.BW) * ((p.Ho + a.BH - 1) / a.BH);
+  const size_t full = 200 * 1024 > extra ? 200 * 1024 - extra : 0;  // one CTA per SM
+  plan->occ = 1;
+  a.stages_a = 0;
+  for (int occ = 2; occ >= 1; occ--) {
+    const size_t budget = occ == 2 ? (104 * 1024 > extra ? 104 * 1024 - extra : 0) : full;  // operand rings
+    // layers with <= 2 tiles per CTA gain nothing from deep rings or resident weights; a small footprint
+    // lets the NEXT kernel's CTAs (PDL / sibling branches) become resident while this one drains
+    const bool small = m_tiles * a.n_tiles <= 2 * num_sms;
+    if (occ == 2 && (a.n_tile > 64 || max_occ < 2)) continue;
+    // keep the whole weight matrix in smem when it leaves room for >= 3 activation slabs: removes the
+    // weight re-fetch per tile
+    a.b_resident = (a.n_tiles == 1 && b_all + 3 * (size_t)a.a_stride <= budget) ? 1 : 0;
+    // resident weights at one CTA/SM beat re-fetched weights at two CTAs/SM
+    if (occ == 2 && !plan_small() && !small && !a.b_resident && a.n_tiles == 1 && b_all + 3 * (size_t)a.a_stride <= full) continue;
+    if (a.b_resident) {
+      a.stages_a = (int)std::min<size_t>(a.mode != TC_TAP ? (a.chunks > 1 ? 8 : 6) : TC_MAX_STAGES, (budget - b_all) / a.a_stride);
+      a.stages_b = 0;
+    } else if (a.mode != TC_TAP) {
+      // A slab serves 9 B slabs: a short A ring and as many weight slabs as fit
+      a.stages_a = (int)std::min<size_t>(3, std::max<size_t>(2, (budget / 3) / a.a_stride));
+      const size_t rest = budget > (size_t)a.stages_a * a.a_stride ? budget - (size_t)a.stages_a * a.a_stride : 0;
+      a.stages_b = (int)std::min<size_t>(TC_MAX_STAGES, rest / a.b_stride);
+    } else {
+      a.stages_a = a.stages_b = (int)std::min<size_t>(8, budget / (a.a_stride + a.b_stride));
+    }
+    const size_t rings = (size_t)a.stages_a * a.a_stride + (a.b_resident ? b_all : (size_t)a.stages_b * a.b_stride);
+    a.w2_off = (uint32_t)rings;
+    plan->smem = rings + extra + 1024;
+    const bool fits = a.stages_a >= 2 && (a.b_resident || a.stages_b >= ((occ == 2 && a.mode != TC_TAP) ? 3 : 2)) && rings <= budget;
+    if (fits && (occ == 1 || small || a.stages_a >= 3 || plan_small())) { plan->occ = occ; break; }
+    if (occ == 1) a.stages_a = 0;  // reported below
+  }
+  plan->small = m_tiles * a.n_tiles <= 2 * num_sms;
+  plan->grid = num_sms * plan->occ;
+  if (plan_small() && plan->occ == 2) plan->grid = num_sms;  // the SM's other half belongs to the other stream's kernel
+  return !(a.stages_a < 2 || (!a.b_resident && a.stages_b < 2));
 }
 
 TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
@@ -752,51 +898,7 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
     }
     a.wpk = plan->wpk;
   }
-  // Two CTAs per SM (each <= ~100 KiB smem) double the tiles in flight per SM and hide the producer -> MMA ->
-  // epilogue hand-off latencies of the HBM-bound high-resolution layers; they need n_tile <= 64 (the register budget of
-  // two 288-thread CTAs leaves room for 32 accumulator registers per thread).  Layers whose resident weights or wide N
-  // tiles do not fit run one CTA per SM with the full budget.
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  const size_t b_all = (size_t)a.ksteps * a.b_stride;
-  const int m_tiles = plan->flat ? (p.B * p.Ho * p.Wo + 127) / 128
-                                 : p.B * ((p.Wo + a.BW - 1) / a.BW) * ((p.Ho + a.BH - 1) / a.BH);
-  plan->occ = 1;
-  for (int occ = 2; occ >= 1; occ--) {
-    const size_t budget = occ == 2 ? 104 * 1024 : 200 * 1024;  // operand rings
-    // layers with <= 2 tiles per CTA gain nothing from deep rings or resident weights; a small footprint
-    // lets the NEXT kernel's CTAs (PDL / sibling branches) become resident while this one drains
-    const bool small = m_tiles * a.n_tiles <= 2 * num_sms;
-    if (occ == 2 && a.n_tile > 64) continue;
-    // keep the whole weight matrix in smem when it leaves room for >= 3 activation slabs: removes the
-    // weight re-fetch per tile
-    a.b_resident = (a.n_tiles == 1 && b_all + 3 * (size_t)a.a_stride <= budget) ? 1 : 0;
-    // resident weights at one CTA/SM beat re-fetched weights at two CTAs/SM
-    if (occ == 2 && !plan_small() && !small && !a.b_resident && a.n_tiles == 1 && b_all + 3 * (size_t)a.a_stride <= 200 * 1024) continue;
-    if (a.b_resident) {
-      a.stages_a = (int)std::min<size_t>(a.mode != TC_TAP ? (a.chunks > 1 ? 8 : 6) : TC_MAX_STAGES, (budget - b_all) / a.a_stride);
-      a.stages_b = 0;
-      plan->smem = (size_t)a.stages_a * a.a_stride + b_all + 1024;
-    } else if (a.mode != TC_TAP) {
-      // A slab serves 9 B slabs: a short A ring and as many weight slabs as fit
-      a.stages_a = (int)std::min<size_t>(3, std::max<size_t>(2, (budget / 3) / a.a_stride));
-      const size_t rest = budget > (size_t)a.stages_a * a.a_stride ? budget - (size_t)a.stages_a * a.a_stride : 0;
-      a.stages_b = (int)std::min<size_t>(TC_MAX_STAGES, rest / a.b_stride);
-      plan->smem = (size_t)a.stages_a * a.a_stride + (size_t)a.stages_b * a.b_stride + 1024;
-    } else {
-      a.stages_a = a.stages_b = (int)std::min<size_t>(8, budget / (a.a_stride + a.b_stride));
-      plan->smem = (size_t)a.stages_a * (a.a_stride + a.b_stride) + 1024;
-    }
-    const bool fits = a.stages_a >= 2 && (a.b_resident || a.stages_b >= ((occ == 2 && a.mode != TC_TAP) ? 3 : 2)) &&
-                      (size_t)a.stages_a * a.a_stride + (a.b_resident ? b_all : (size_t)a.stages_b * a.b_stride) <= budget;
-    if (fits && (occ == 1 || small || a.stages_a >= 3 || plan_small())) { plan->occ = occ; break; }
-    if (occ == 1) a.stages_a = 0;  // reported below
-  }
-  if (a.stages_a < 2 || (!a.b_resident && a.stages_b < 2)) {
+  if (!tc_size_rings(plan, 0, tc_ctas_per_sm(a.n_tile / 16, 0))) {
     if (err) *err = "tile does not fit in shared memory";
     delete plan;
     return nullptr;
@@ -820,18 +922,80 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
       return nullptr;
     }
   }
-  plan->grid = num_sms * plan->occ;
-  if (plan_small() && plan->occ == 2) plan->grid = num_sms;  // the SM's other half belongs to the other stream's kernel
-  plan->small = m_tiles * a.n_tiles <= 2 * num_sms;
+  return plan;
+}
+
+// The fold instantiations, as (this conv's n_tile, the 1x1's Cout) / 16: the pairs of the YOLOv8 / YOLOv11 detection
+// models.  A pair without one stays unfolded; 256 -> 128 and 160 -> 160 are left out because their fragments and
+// accumulators spill even at one CTA per SM (the 1x1 passes of 64 / 80 columns need the fragments of all 256 / 160
+// input channels live through every pass).
+static void (*tc_fold_kernel(int nt16, int n2_16))(TcArgs) {
+#define YB_FOLD_KERNEL(N, N2) \
+  if (nt16 == N && n2_16 == N2) return conv_tc_kernel<N, N2>;
+  YB_FOLD_KERNEL(2, 2)    // 32 -> 32: v8n / v11n model.1 -> model.2.cv1
+  YB_FOLD_KERNEL(4, 4)    // 64 -> 64: model.1 / 3 -> C2f / C3k2 cv1, the DFL box tails of c2 = 64
+  YB_FOLD_KERNEL(5, 4)    // 80 -> 64: DFL box tails of c2 = 80 (v8x)
+  YB_FOLD_KERNEL(5, 5)    // 80 -> 80: class tails of c3 = 80 (v8n, v11n)
+  YB_FOLD_KERNEL(8, 5)    // 128 -> 80: class tails of c3 = 128 (v8s, v11s)
+  YB_FOLD_KERNEL(8, 8)    // 128 -> 128: model.5 -> model.6.cv1 (v8n), model.3 -> model.4.cv1 (v8s)
+#undef YB_FOLD_KERNEL
+  return nullptr;
+}
+
+TcConvPlan* tc_fold_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, std::string* err) {
+  const TcArgs &a1 = pa->args, &a2 = pb->args;
+  const ConvParams &p1 = pa->p, &p2 = pb->p;
+  auto fail = [&](const std::string& m) -> TcConvPlan* { if (err) *err = m; return nullptr; };
+  if (a1.n_tiles != 1) return fail("the producer splits Cout over " + std::to_string(a1.n_tiles) + " N tiles");
+  if (a1.epi_mode != EPI_STORE || p1.res.base || (p1.act != ACT_SILU && p1.act != ACT_NONE))
+    return fail("the producer is not a plain conv that stores its output");
+  if (!pb->flat || a2.n_tiles != 1 || p2.res.base || p2.Cin != p1.Cout || p2.Cout > TC_FOLD_BIAS)
+    return fail("the consumer is not a single-tile 1x1 over the producer's channels");
+  const int nt16 = a1.n_tile / 16, n2_16 = p2.Cout / 16;
+  // column passes of at most 80: the second accumulator stays within the register budget of the producer's tile
+  const int f16 = tc_fold_pass16(n2_16);
+  TcConvPlan* plan = new TcConvPlan(*pa);
+  plan->wpk = nullptr;  // both slab sets belong to the two conv plans
+  plan->fold16 = f16;
+  TcArgs& a = plan->args;
+  a.w2 = a2.wpk; a.bias2 = p2.bias;
+  a.w2_bytes = (uint32_t)(a2.ksteps * a2.b_stride);
+  a.b2_stride = a2.b_stride; a.sbo_b2 = a2.sbo_b; a.layout_b2 = a2.layout_b;
+  a.BK2 = a2.BK; a.n2 = p2.Cout; a.act1 = a1.act;
+  // the epilogue is the 1x1's
+  a.out = a2.out; a.out_pitch = a2.out_pitch; a.out_coff = a2.out_coff;
+  a.res = nullptr; a.res_pitch = a.res_coff = 0;
+  a.act = a2.act;
+  a.epi_mode = a2.epi_mode;
+  a.dA = a2.dA; a.dCtot = a2.dCtot; a.da0 = a2.da0; a.dch0 = a2.dch0; a.dWl = a2.dWl; a.dHW = a2.dHW; a.dstride = a2.dstride;
+  if (!tc_size_rings(plan, a.w2_bytes, tc_ctas_per_sm(nt16, n2_16))) {
+    delete plan;
+    return fail("the producer's rings and the 1x1's " + std::to_string(a.w2_bytes / 1024) + " KiB of weights do not fit in shared memory");
+  }
+  void (*kernel)(TcArgs) = tc_fold_kernel(nt16, n2_16);
+  if (!kernel || (a2.epi_mode == EPI_DFL_BOX && f16 != 4)) {
+    delete plan;
+    return fail("no fold instantiation for " + std::to_string(a1.n_tile) + " -> " + std::to_string(p2.Cout) + " channels");
+  }
+  plan->kernel = kernel;
+  cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  const cudaError_t ce = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 202 * 1024);
+  if (ce != cudaSuccess) {
+    delete plan;
+    return fail(std::string("cudaFuncSetAttribute(conv_tc_kernel) failed: ") + cudaGetErrorString(ce));
+  }
   return plan;
 }
 
 std::string tc_conv_plan_describe(const TcConvPlan* plan) {
   const TcArgs& a = plan->args;
-  char buf[256];
-  snprintf(buf, sizeof(buf), "mode %d BK %d chunks %d n_tile %d x%d stages a/b %d/%d resident %d occ %d threads %d smem %zu KiB grid %d",
-           a.mode, a.BK, a.chunks, a.n_tile, a.n_tiles, a.stages_a, a.stages_b, a.b_resident, plan->occ, TC_THREADS, plan->smem / 1024,
-           plan->grid);
+  char buf[320];
+  int n = snprintf(buf, sizeof(buf), "mode %d BK %d chunks %d n_tile %d x%d stages a/b %d/%d resident %d occ %d threads %d smem %zu KiB grid %d",
+                   a.mode, a.BK, a.chunks, a.n_tile, a.n_tiles, a.stages_a, a.stages_b, a.b_resident, plan->occ, TC_THREADS,
+                   plan->smem / 1024, plan->grid);
+  if (plan->fold16 && n > 0 && n < (int)sizeof(buf))
+    snprintf(buf + n, sizeof(buf) - n, " fold 1x1 %d->%d BK %d pass %d w2 %u KiB", a.n_tile, a.n2, a.BK2, 16 * plan->fold16,
+             a.w2_bytes / 1024);
   return buf;
 }
 
@@ -1344,11 +1508,6 @@ struct StemArgs {
   int tiles_w, tiles_h, total_tiles;
   uint64_t m_tpi, m_tw;  // magic numbers for / tiles_per_img and / tiles_w (fdiv)
 };
-
-__device__ __forceinline__ uint32_t pack_h2(float x, float y) {
-  const __half2 h = __floats2half2_rn(x, y);
-  return *reinterpret_cast<const uint32_t*>(&h);
-}
 
 // four input columns col .. col+3 (col even, may be -2) of one row as 4 halves; `lo_ok` = col >= 0
 template <int DT>

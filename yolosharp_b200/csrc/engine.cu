@@ -74,7 +74,9 @@ struct OpDesc {
   EpiDecode dec;       // conv: fused Detect-tail epilogue (tensor-core path)
   bool fused = false;  // decode op: its work is done by the producing convs' epilogues
   TcBneckPlan* bneck = nullptr;  // conv: fused Bottleneck that also computes the previous op (its input) in smem
-  bool absorbed = false;         // conv: computed inside the next op's fused Bottleneck launch; launches nothing
+  bool absorbed = false;         // conv: computed inside the next op's fused launch (Bottleneck or fold); launches nothing
+  TcConvPlan* fold = nullptr;    // 1x1 conv: plan that also computes the previous op, its input never leaving registers
+  bool folded = false;           // conv: absorbed into the next op's fold
 };
 
 struct HostTensor {
@@ -737,7 +739,7 @@ static int run_ops(yb_engine* e, const void* in, int in_dtype, int B, float* out
           rc = tc_bneck_launch(op.bneck, B, e->tile_ctr ? e->tile_ctr + i : nullptr, s);
         } else if (op.use_tc) {
           TcChain ch;
-          const bool chained = e->chain != 0 && only < 0;
+          const bool chained = e->chain != 0 && only < 0 && !op.fold;
           if (chained) {
             ch.done_ctr = e->done_ctr + i * (size_t)e->cfg.max_batch;
             if (op.dep_op >= 0) {
@@ -745,7 +747,8 @@ static int run_ops(yb_engine* e, const void* in, int in_dtype, int B, float* out
               ch.dep_expect = tc_conv_rows_per_image(e->ops[op.dep_op].plan);
             }
           }
-          rc = tc_conv_launch(op.plan, B, out_pred, e->tile_ctr ? e->tile_ctr + i : nullptr, s, chained ? &ch : nullptr);
+          rc = tc_conv_launch(op.fold ? op.fold : op.plan, B, out_pred, e->tile_ctr ? e->tile_ctr + i : nullptr, s,
+                              chained ? &ch : nullptr);
         } else {
           rc = launch_conv_generic<T>(conv_params(e, op, B), s);
         }
@@ -895,6 +898,7 @@ void yb_destroy(yb_engine* e) {
   cudaSetDevice(e->cfg.device);
   for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
   for (auto& op : e->ops) if (op.bneck) tc_bneck_plan_destroy(op.bneck);
+  for (auto& op : e->ops) if (op.fold) tc_conv_plan_destroy(op.fold);
   for (auto& op : e->ops) if (op.plan) tc_conv_plan_destroy(op.plan);
   for (void* p : e->dev_allocs) cudaFree(p);
   if (e->arena) cudaFree(e->arena);
@@ -1055,6 +1059,33 @@ int32_t yb_finalize_weights(yb_engine* e) {
     a.absorbed = true;
     if (getenv("YB_DEBUG_PLANS")) fprintf(stderr, "[plan] %-30s %s (absorbs %s)\n", b.name.c_str(), tc_bneck_plan_describe(b.bneck).c_str(), a.name.c_str());
   }
+  // 1x1 fold: a tensor-core conv that stores its output, whose output buffer has exactly one reader, the next op of the
+  // same lane, a 1x1 s1 tensor-core conv: that 1x1 runs inside the conv's launch on the accumulator registers of each
+  // tile (tc_fold_plan_create decides whether the pair fits).  The producer stays in the op list, launches nothing and
+  // keeps its arena buffer for yb_debug_read_activation.  YB_NO_FOLD1X1=1 turns the pass off.
+  const char* no_fold = getenv("YB_NO_FOLD1X1");
+  for (size_t i = 1; i + 1 < e->ops.size() && !(no_fold && atoi(no_fold)); i++) {
+    OpDesc &a = e->ops[i], &b = e->ops[i + 1];
+    if (a.type != OP_CONV || b.type != OP_CONV || !a.use_tc || !b.use_tc || a.absorbed || a.bneck || a.fold || b.bneck) continue;
+    if (a.res.buf >= 0 || a.dec.mode != EPI_STORE || b.k != 1 || b.s != 1 || b.res.buf >= 0 || a.lane != b.lane) continue;
+    if (b.in.buf != a.out.buf || b.in.coff != a.out.coff || b.in.C != a.out.C) continue;
+    bool single = true;
+    for (size_t j = 0; j < e->ops.size(); j++) {
+      const OpDesc& o = e->ops[j];
+      if (j == i || j == i + 1) continue;
+      for (const VRef* r : {&o.in, &o.out, &o.res, &o.out2, &o.out3, &o.cls, &o.coef})
+        if (r->buf == a.out.buf) single = false;
+    }
+    if (!single) continue;
+    std::string err;
+    b.fold = tc_fold_plan_create(a.plan, b.plan, &err);
+    if (!b.fold) {
+      if (getenv("YB_DEBUG_PLANS")) fprintf(stderr, "[plan] %-30s fold refused (%s): %s\n", b.name.c_str(), a.name.c_str(), err.c_str());
+      continue;
+    }
+    a.absorbed = a.folded = true;
+    if (getenv("YB_DEBUG_PLANS")) fprintf(stderr, "[plan] %-30s %s (folds %s)\n", b.name.c_str(), tc_conv_plan_describe(b.fold).c_str(), a.name.c_str());
+  }
   // Layer chaining: inside a lane, a tensor-core conv whose stream predecessor is a tensor-core conv that stores an NHWC
   // tensor starts its tiles per image, as soon as the predecessor has stored that image (per-image counters), instead
   // of waiting for the predecessor's whole grid.  Completion per image is monotone along the lane (every op waits for
@@ -1070,10 +1101,10 @@ int32_t yb_finalize_weights(yb_engine* e) {
       if ((op.type == OP_DECODE && op.fused) || op.absorbed) continue;  // launches nothing
       const int lane = (e->cfg.flags & YB_FLAG_NO_CONCURRENCY) ? 0 : op.lane;
       const int pv = prev_in_lane[lane];
-      // fused Bottlenecks neither wait on nor publish per-image counters: they keep the grid-wide dependency both ways
-      if (op.type == OP_CONV && op.use_tc && !op.bneck && pv >= 0) {
+      // fused Bottlenecks and folds neither wait on nor publish per-image counters: they keep the grid-wide dependency both ways
+      if (op.type == OP_CONV && op.use_tc && !op.bneck && !op.fold && pv >= 0) {
         const OpDesc& pr = e->ops[pv];
-        if (pr.type == OP_CONV && pr.use_tc && !pr.bneck && pr.dec.mode == EPI_STORE) op.dep_op = pv;
+        if (pr.type == OP_CONV && pr.use_tc && !pr.bneck && !pr.fold && pr.dec.mode == EPI_STORE) op.dep_op = pv;
       }
       prev_in_lane[lane] = (int)i;
     }
@@ -1429,7 +1460,7 @@ int32_t yb_debug_read_activation(yb_engine* e, int32_t op_index, int32_t batch, 
   if (n > host_capacity) { set_error("yb_debug_read_activation: host buffer too small"); return YB_ERR_INVALID_ARG; }
   int rc = 0;
   if (op.absorbed) {
-    // The fused Bottleneck kept this op's output in shared memory only: materialise it now into the op's own arena
+    // The fused Bottleneck (shared memory) or the fold (registers) never stored this op's output: materialise it now into the op's own arena
     // buffer with the fp16 CUDA-core twin (same fp16-rounded weights).  Its input slice is still what the last forward
     // read, because arena buffers are never reused within a forward.
     rc = launch_conv_generic<__half>(conv_params(e, op, batch), 0);
@@ -1515,10 +1546,19 @@ int32_t yb_op_cost(const yb_engine* e, int32_t i, int32_t batch, double* flops, 
       *bytes -= vbytes(op.in);
       *bytes += (double)batch * 3 * e->cfg.height * e->cfg.width * e->esize;
     }
-    if (op.absorbed) *bytes = 0;  // moved by the fused Bottleneck launch of the next op
+    if (op.absorbed) *bytes = 0;  // moved by the fused launch of the next op
     if (op.bneck) {               // reads the block input (once, also as the shortcut) and both weight sets
       const OpDesc& pa = e->ops[i - 1];
       *bytes = vbytes(pa.in) + vbytes(op.out) + (double)(pa.cout * pa.cin + op.cout * op.cin) * 9 * e->esize;
+    }
+    // A folded producer launches nothing and reports no work of its own (yb_op_kind 6, like a fused Detect decode); its
+    // FLOPs are the folding 1x1's, whose launch reads the producer's input and both weight sets and stores its output.
+    if (op.folded) *flops = 0;
+    if (op.fold) {
+      const OpDesc& pa = e->ops[i - 1];
+      const BufDesc& pb = e->bufs[pa.out.buf];
+      *flops += 2.0 * batch * pb.H * pb.W * pa.cout * pa.cin * pa.k * pa.k;
+      *bytes += vbytes(pa.in) + (double)pa.cout * pa.cin * pa.k * pa.k * e->esize - vbytes(op.in);
     }
   } else if (op.type == OP_DECODE) {
     *bytes = vbytes(op.in) + vbytes(op.cls) + vbytes(op.coef) +
@@ -1656,7 +1696,7 @@ int32_t yb_op_kind(const yb_engine* e, int32_t i) {
   if (!e || i < 0 || i >= (int32_t)e->ops.size()) return -1;
   const OpDesc& op = e->ops[i];
   switch (op.type) {
-    case OP_CONV: return (i == 0 && e->has_stem_tc) ? 2 : (op.use_tc ? 0 : 1);
+    case OP_CONV: return (i == 0 && e->has_stem_tc) ? 2 : (op.folded ? 6 : (op.use_tc ? 0 : 1));
     case OP_DWCONV: return 3;
     case OP_POOL: return 4;
     case OP_UPSAMPLE: return 5;

@@ -196,6 +196,50 @@ __device__ __forceinline__ void wg_mma_n(float* d, uint32_t a_lo, uint32_t a_hi,
   }
 }
 
+// wgmma with the A operand in registers (m64nNk16, f16 -> f32).  `a` is the k16 fragment of this thread, four f16 pairs
+// in the layout of an m64n16 accumulator: a[0] = row 16w + l/4, columns 2(l%4) + {0, 1}; a[1] = row + 8, same columns;
+// a[2], a[3] = the same rows, columns + 8.  So the f32 accumulator of an m64nN wgmma, rounded to f16 pairs, is the A
+// operand of N / 16 k16 steps of the next GEMM (conv_tc.cu, tc_fold).
+template <int N>
+__device__ __forceinline__ void wgmma_f16_rs(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_f16_rs<16>(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_f16_rs<32>(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_f16_rs<64>(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+
+// The register-A counterpart of wg_mma_n: 64 x (16 * NT16) x k16 as the fewest instructions of N = 64 / 32 / 16.
+template <int NT16, int C16 = 0>
+__device__ __forceinline__ void wg_mma_rs_n(float* d, const uint32_t* a, uint32_t b_lo, uint32_t b_hi, uint32_t b_row16,
+                                            uint32_t scale_d) {
+  if constexpr (C16 < NT16) {
+    constexpr int R = NT16 - C16;
+    constexpr int W = R >= 4 ? 4 : (R >= 2 ? 2 : 1);
+    wgmma_f16_rs<W * 16>(d + C16 * 8, a, desc64(b_lo + (uint32_t)(C16 * 16) * b_row16, b_hi), scale_d);
+    wg_mma_rs_n<NT16, C16 + W>(d, a, b_lo, b_hi, b_row16, scale_d);
+  }
+}
+
 // Run `f(integral_constant<NT16>)` for a runtime n_tile (a multiple of 16, <= 256).
 template <int NT16 = 1, class F>
 inline void dispatch_nt16(int nt16, F&& f) {
