@@ -511,6 +511,23 @@ int32_t yb_debug_bneck_f16(const void* x, int32_t batch, int32_t height, int32_t
                            const void* w_a, const float* bias_a, int32_t cmid, const void* w_b, const float* bias_b, int32_t cout,
                            int32_t shortcut, void* out, int32_t out_pitch, int32_t out_coff, char* desc, int32_t desc_capacity);
 
+/* debug: ONE pass of the TF32 tensor-core training convolution (csrc/conv_tf32.cu) on caller-owned device buffers, through
+ * the same host functions the training step calls; synchronises before it returns.  Op-level tests compare it with a
+ * float64 convolution.  k 1 or 3, stride 1 or 2, pad k / 2, cin and cout multiples of 8.
+ *   pass 0  forward:          out (n, Ho, Wo, cout) = conv(x, w) + bias (bias may be NULL)
+ *   pass 1  data gradient:    out (n, height, width, cin) = dx from dz (n, Ho, Wo, cout); height, width even at stride 2
+ *   pass 2  weight gradient:  out (cout, cin, k, k) = dw from x and dz
+ *   x       fp32 NHWC (n, height, width, cin); x_pitch 0 = dense, else the element stride between pixels, x pointing at the
+ *           first channel of the view (16-byte aligned, x_pitch a multiple of 4); passes 0 and 2 only
+ *   w       fp32 (cout, cin, k, k), the checkpoint layout;  workspace: yb_conv_tc_workspace_bytes(...) bytes
+ *   desc    receives one line per kernel launch with the values that were launched (tf_conv_kernel: BK, chunks,
+ *           n_tile x n_tiles, BW x BH, in_stride, flat, ntaps, occ, stages, grid; tf_wgrad_kernel: halo, tpc, nb,
+ *           co_tiles, ci_tiles, co_blocks, splits, pix_tiles, b_stages, grid), or NULL
+ * A shape the kernels or their planners do not take returns YB_ERR_SHAPE with the reason. */
+int32_t yb_debug_conv_tf32(int32_t pass, const float* x, int32_t x_pitch, const float* dz, const float* w, const float* bias,
+                           int32_t n, int32_t height, int32_t width, int32_t cin, int32_t cout, int32_t k, int32_t stride,
+                           float* out, void* workspace, int64_t workspace_bytes, char* desc, int32_t desc_capacity);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,7 +5,7 @@ torch.nn.functional.conv2d + autograd in fp32 (TF32 disabled) on the same inputs
 Tolerance: TF32 keeps 10 mantissa bits of every operand (products exact in fp32, fp32 accumulation), so an output that
 sums K products of O(1) terms carries an absolute error of about 2^-11 * sqrt(K) * rms; the tests bound the error by
 1e-2 of the output's rms scale (max over all elements; observed 2e-3 .. 6e-3) (observed values are printed) - the tolerance class libtorch's own TF32 convolutions
-have against fp32."""
+have against fp32.  Element-wise bounds, integer bit-exactness and the stem are in test_gpu_conv_tf32_ops.py."""
 import pytest
 import torch
 
@@ -72,53 +72,6 @@ def test_conv_tc_forward_dgrad_wgrad(shape):
     z32 = E.conv_forward(x, w, b, s, k // 2)
     dx32, dw32 = E.conv_backward(x, dz, w, s, k // 2)
     assert _rel(z, z32) < 1e-2 and _rel(dx, dx32) < 1e-2 and _rel(dw, dw32) < 1e-2
-
-
-@gpu
-def test_conv_tc_exact_on_tf32_representable_inputs():
-    """With operands that are exactly representable in TF32 (small integers) and sums that stay exact in fp32, the
-    tensor-core kernels must agree with fp32 bit for bit: separates layout / indexing errors from rounding."""
-    import yolosharp_b200.engine as E
-    g = torch.Generator().manual_seed(1)
-    for shape in [(2, 20, 20, 32, 48, 3, 1), (2, 16, 16, 16, 24, 3, 2), (1, 12, 12, 64, 64, 1, 1)]:
-        N, H, W, Cin, Cout, k, s = shape
-        x = torch.randint(-4, 5, (N, H, W, Cin), generator=g).float().cuda()
-        w = torch.randint(-3, 4, (Cout, Cin, k, k), generator=g).float().cuda()
-        Ho, Wo = (H + 2 * (k // 2) - k) // s + 1, (W + 2 * (k // 2) - k) // s + 1
-        dz = torch.randint(-2, 3, (N, Ho, Wo, Cout), generator=g).float().cuda()
-        ws = E.ConvWorkspace(x.device)
-        z = E.conv_forward_tc(x, w, None, s, k // 2, ws=ws)
-        dx, dw = E.conv_backward_tc(x, dz, w, s, k // 2, ws=ws)
-        z32 = E.conv_forward(x, w, None, s, k // 2)
-        dx32, dw32 = E.conv_backward(x, dz, w, s, k // 2)
-        assert torch.equal(z, z32), shape
-        assert torch.equal(dx, dx32), shape
-        assert torch.equal(dw, dw32), shape
-
-
-@gpu
-@pytest.mark.parametrize("N,H,W,C,xc", [(2, 64, 96, 16, 3), (1, 32, 32, 32, 8), (2, 40, 24, 80, 8), (1, 640, 640, 32, 8)])
-def test_stem_conv_forward_and_wgrad_vs_torch(N, H, W, C, xc):
-    """The fp32 CUDA-core stem kernels (yb_stem_conv_*): x with 3 or 8 (zero-padded) channels per pixel."""
-    import yolosharp_b200.engine as E
-    g = torch.Generator().manual_seed(5)
-    x3 = torch.randn(N, H, W, 3, generator=g)
-    w = torch.randn(C, 3, 3, 3, generator=g) / 27 ** 0.5
-    dz = torch.randn(N, H // 2, W // 2, C, generator=g)
-    xt = x3.permute(0, 3, 1, 2).contiguous().cuda()
-    wt = w.clone().cuda().requires_grad_(True)
-    old = torch.backends.cudnn.allow_tf32
-    torch.backends.cudnn.allow_tf32 = False
-    try:
-        zt = torch.nn.functional.conv2d(xt, wt, None, stride=2, padding=1)
-        zt.backward(dz.permute(0, 3, 1, 2).contiguous().cuda())
-    finally:
-        torch.backends.cudnn.allow_tf32 = old
-    x = torch.nn.functional.pad(x3, (0, xc - 3)).contiguous().cuda()
-    z = E.stem_conv_forward(x, w.cuda())
-    dw = E.stem_conv_backward_weight(x, dz.cuda(), w.shape)
-    torch.testing.assert_close(z, zt.detach().permute(0, 2, 3, 1), rtol=1e-4, atol=1e-5)
-    assert _rel(dw, wt.grad) < 1e-4
 
 
 @gpu

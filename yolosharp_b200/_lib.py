@@ -123,6 +123,8 @@ SIGNATURES = {
                                   c_i32, c_f32, c_vp, c_vp, c_i32]),
     "yb_debug_bneck_f16": (c_i32, [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_i32, c_vp,
                                    c_i32, c_i32, c_vp, c_i32]),
+    "yb_debug_conv_tf32": (c_i32, [c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp,
+                                   C.c_int64, c_vp, c_i32]),
 }
 
 _lib = None

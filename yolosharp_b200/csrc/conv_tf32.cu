@@ -271,7 +271,8 @@ struct TfLaunch {
   bool flat;         // 1x1 stride 1, dense output: flatten the batch into one position dimension
 };
 
-static int tf_conv_launch(const TfLaunch& L, cudaStream_t s) {
+// desc: when set, receives one line describing the launch (yb_debug_conv_tf32)
+static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) {
   TfEncodeFn encode = tf_encode_fn();
   if (!encode) { set_error("cuTensorMapEncodeTiled entry point not found"); return YB_ERR_CUDA; }
   TfArgs a;
@@ -355,6 +356,13 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s) {
     attr_set[a.n_tile / 16] = true;
   }
   const int grid = std::min(a.total_tiles, occ * tf_num_sms());
+  if (desc) {
+    char line[256];
+    snprintf(line, sizeof(line), "%stf_conv_kernel BK %d chunks %d n_tile %d x%d BW %d BH %d in_stride %d flat %d ntaps %d occ %d stages %d grid %d",
+             desc->empty() ? "" : "\n", a.BK, a.chunks, a.n_tile, a.n_tiles, a.BW, a.BH, a.in_stride, L.flat ? 1 : 0, a.ntaps, occ,
+             a.stages, grid);
+    *desc += line;
+  }
   YB_CUDA_CHECK(launch_pdl(kernel, dim3(grid), dim3(TF_THREADS), smem, s, a));
   return 0;
 }
@@ -366,7 +374,8 @@ static bool tf_shape_ok(int Cin, int Cout, int k, int stride, int pad) {
 }
 
 int tf_conv_forward(const float* x, const float* w, const float* bias, int N, int H, int W, int Cin, int Cout, int k, int stride,
-                    int pad, float* z, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, const float* prepacked) {
+                    int pad, float* z, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, const float* prepacked,
+                    std::string* desc = nullptr) {
   if (x_pitch && (x_pitch < Cin || x_pitch % 4 || ((uintptr_t)x & 15))) { set_error("tf32 conv: input view must be 16-byte aligned with a pitch multiple of 4"); return YB_ERR_SHAPE; }
   if (!tf_shape_ok(Cin, Cout, k, stride, pad)) { set_error("tf32 conv: channels must be multiples of 8, k in {1,3}, stride in {1,2}, pad = k/2"); return YB_ERR_SHAPE; }
   const size_t wn = (size_t)Cout * Cin * k * k;
@@ -385,11 +394,12 @@ int tf_conv_forward(const float* x, const float* w, const float* bias, int N, in
   L.ntaps = k * k;
   for (int t = 0; t < k * k; t++) { L.dh[t] = t / k - pad; L.dw[t] = t % k - pad; L.slab[t] = t; }
   L.flat = (k == 1 && stride == 1);
-  return tf_conv_launch(L, s);
+  return tf_conv_launch(L, s, desc);
 }
 
 int tf_conv_backward_data(const float* dz, const float* w, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
-                          float* dx, float* ws, size_t ws_bytes, cudaStream_t s, const float* prepacked) {
+                          float* dx, float* ws, size_t ws_bytes, cudaStream_t s, const float* prepacked,
+                          std::string* desc = nullptr) {
   if (!tf_shape_ok(Cin, Cout, k, stride, pad) || (stride == 2 && ((H | W) & 1))) {
     set_error("tf32 dgrad: channels must be multiples of 8, k in {1,3}, stride in {1,2} (even size for stride 2), pad = k/2");
     return YB_ERR_SHAPE;
@@ -412,7 +422,7 @@ int tf_conv_backward_data(const float* dz, const float* w, int N, int H, int W, 
     L.ntaps = k * k;
     for (int t = 0; t < k * k; t++) { L.dh[t] = pad - t / k; L.dw[t] = pad - t % k; L.slab[t] = t; }
     L.flat = (k == 1);
-    return tf_conv_launch(L, s);
+    return tf_conv_launch(L, s, desc);
   }
   // stride 2: dx(2a + py, 2b + px) = sum over taps with (py + pad - kh), (px + pad - kw) even of dz(a + (py+pad-kh)/2, b + ...)
   // k = 1 (pad 0): only parity (0,0) receives gradient; the other positions are zero.
@@ -433,7 +443,7 @@ int tf_conv_backward_data(const float* dz, const float* w, int N, int H, int W, 
       L.o_pix = 2LL * Cin; L.o_row = 2LL * W * Cin; L.o_img = (long long)H * W * Cin;
       L.o_off = ((long long)py * W + px) * Cin;
       L.flat = false;
-      const int rc = tf_conv_launch(L, s);
+      const int rc = tf_conv_launch(L, s, desc);
       if (rc) return rc;
     }
   return 0;
@@ -678,7 +688,7 @@ size_t tf_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, in
 }
 
 int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
-                            float* dw, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch) {
+                            float* dw, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, std::string* desc = nullptr) {
   if (x_pitch && (x_pitch < Cin || x_pitch % 4 || ((uintptr_t)x & 15))) { set_error("tf32 wgrad: input view must be 16-byte aligned with a pitch multiple of 4"); return YB_ERR_SHAPE; }
   const int xp = x_pitch ? x_pitch : Cin;
   if (!tf_shape_ok(Cin, Cout, k, stride, pad)) { set_error("tf32 wgrad: channels must be multiples of 8, k in {1,3}, stride in {1,2}, pad = k/2"); return YB_ERR_SHAPE; }
@@ -730,6 +740,12 @@ int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W
   }
   const size_t smem = (size_t)WG_A_STAGES * 4 * WG_BLK + (size_t)a.b_stages * b_stride + 1024;
   const int grid = p.co_tiles * p.ci_tiles * p.tap_groups * p.splits;
+  if (desc) {
+    char line[256];
+    snprintf(line, sizeof(line), "%stf_wgrad_kernel halo %d tpc %d nb %d co_tiles %d ci_tiles %d co_blocks %d splits %d pix_tiles %d b_stages %d grid %d",
+             desc->empty() ? "" : "\n", a.halo, a.tpc, a.nb, a.co_tiles, a.ci_tiles, a.co_blocks, a.splits, a.pix_tiles, a.b_stages, grid);
+    *desc += line;
+  }
   YB_CUDA_CHECK(launch_pdl(tf_wgrad_kernel, dim3(grid), dim3(TF_THREADS), smem, s, a));
   const size_t n = (size_t)Cout * Cin * k * k;
   static bool fold_attr = false;
@@ -984,6 +1000,45 @@ int32_t yb_conv_backward_weight_tc(const float* x, const float* dz, int32_t n, i
   if (!tf_have_dev("yb_conv_backward_weight_tc")) return YB_ERR_NO_DEVICE;
   return tf_conv_backward_weight(x, dz, n, height, width, cin, cout, k, stride, pad, dw, (float*)workspace, (size_t)workspace_bytes,
                                  (cudaStream_t)stream, 0);
+}
+
+int32_t yb_debug_conv_tf32(int32_t pass, const float* x, int32_t x_pitch, const float* dz, const float* w, const float* bias,
+                           int32_t n, int32_t height, int32_t width, int32_t cin, int32_t cout, int32_t k, int32_t stride,
+                           float* out, void* workspace, int64_t workspace_bytes, char* desc, int32_t desc_capacity) {
+  if (pass < 0 || pass > 2) { set_error("yb_debug_conv_tf32: pass must be 0 (forward), 1 (data gradient) or 2 (weight gradient)"); return YB_ERR_INVALID_ARG; }
+  if ((pass != 1 && !x) || (pass != 0 && !dz) || (pass != 2 && !w) || !out || !workspace) {
+    set_error("yb_debug_conv_tf32: null argument");
+    return YB_ERR_INVALID_ARG;
+  }
+  if (n <= 0 || height <= 0 || width <= 0 || cin <= 0 || cout <= 0 || workspace_bytes <= 0 || x_pitch < 0 ||
+      (x_pitch && (pass == 1 || x_pitch < cin || x_pitch % 4 || ((uintptr_t)x & 15)))) {
+    set_error("yb_debug_conv_tf32: bad argument (extent, workspace size, or x_pitch: >= cin, a multiple of 4 on a 16-byte aligned "
+              "x, and 0 for the data gradient)");
+    return YB_ERR_INVALID_ARG;
+  }
+  if (!tf_shape_ok(cin, cout, k, stride, k / 2) || (pass == 1 && stride == 2 && ((height | width) & 1))) {
+    set_error("yb_debug_conv_tf32: shape not supported: channels must be multiples of 8, k in {1,3}, stride in {1,2}, "
+              "even extents for a stride-2 data gradient");
+    return YB_ERR_SHAPE;
+  }
+  if (!tf_have_dev("yb_debug_conv_tf32")) return YB_ERR_NO_DEVICE;
+  std::string d;
+  float* ws = (float*)workspace;
+  const size_t wsb = (size_t)workspace_bytes;
+  int rc;
+  if (pass == 0)
+    rc = tf_conv_forward(x, w, bias, n, height, width, cin, cout, k, stride, k / 2, out, ws, wsb, 0, x_pitch, nullptr, &d);
+  else if (pass == 1)
+    rc = tf_conv_backward_data(dz, w, n, height, width, cin, cout, k, stride, k / 2, out, ws, wsb, 0, nullptr, &d);
+  else
+    rc = tf_conv_backward_weight(x, dz, n, height, width, cin, cout, k, stride, k / 2, out, ws, wsb, 0, x_pitch, &d);
+  const cudaError_t ce = cudaDeviceSynchronize();
+  if (!rc && ce != cudaSuccess) {
+    set_error(std::string("yb_debug_conv_tf32: kernel failed: ") + cudaGetErrorString(ce));
+    rc = YB_ERR_CUDA;
+  }
+  if (desc && desc_capacity > 0) snprintf(desc, (size_t)desc_capacity, "%s", d.c_str());
+  return rc;
 }
 
 int32_t yb_stem_conv_forward_f32(const float* x, int32_t x_channels, const float* w, int32_t n, int32_t height, int32_t width,

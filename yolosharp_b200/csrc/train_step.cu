@@ -30,9 +30,11 @@ namespace yb {
 
 // entry points of the other translation units this step is made of
 int tf_conv_forward(const float* x, const float* w, const float* bias, int N, int H, int W, int Cin, int Cout, int k, int stride,
-                    int pad, float* z, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, const float* prepacked);
+                    int pad, float* z, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, const float* prepacked,
+                    std::string* desc = nullptr);
 int tf_conv_backward_data(const float* dz, const float* w, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
-                          float* dx, float* ws, size_t ws_bytes, cudaStream_t s, const float* prepacked);
+                          float* dx, float* ws, size_t ws_bytes, cudaStream_t s, const float* prepacked,
+                          std::string* desc = nullptr);
 struct TfPackDesc { long long off, chunk0; int cout, cin, taps, pad_; };
 long long tf_pack_chunks(int cout, int cin, int taps);
 int tf_pack_all(const float* P, float* WF, float* WB, const TfPackDesc* dev_descs, int nd, long long total_chunks, cudaStream_t s);
@@ -41,7 +43,7 @@ int detection_loss_launch_dev(const float* boxes, const float* scores, int B, in
                               int n_max, int topk, float hyp_box, float hyp_cls, float hyp_dfl, float* loss_items, float* grad_boxes,
                               float* grad_scores, unsigned char* fg_out, int* gt_idx_out, float* tscore_out, cudaStream_t s);
 int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
-                            float* dw, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch);
+                            float* dw, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, std::string* desc = nullptr);
 size_t tf_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, int stride);
 int stem3_forward(const float* x, int xc, const float* w, int N, int H, int W, int C, float* z, cudaStream_t s);
 int stem3_backward_weight(const float* x, int xc, const float* dz, int N, int H, int W, int C, float* dw, float* ws, size_t ws_bytes,

@@ -535,6 +535,35 @@ def debug_bneck_f16(x, w_a, bias_a, w_b, bias_b, out, shortcut=True, x_coff=0, o
     return desc.value.decode()
 
 
+def debug_conv_tf32(pass_, out, w=None, x=None, dz=None, bias=None, stride=1, workspace=None):
+    """yb_debug_conv_tf32: one pass of the TF32 training conv on caller buffers -> the launch descriptions (one per line).
+    pass_ 0: out (N, Ho, Wo, Cout) = conv(x, w) + bias; 1: out (N, H, W, Cin) = dx from dz; 2: out (Cout, Cin, k, k) = dw.
+    x (N, H, W, Cin) fp32 NHWC, dense or a channel slice x = buf[..., c0:c0 + Cin] of a wider buffer (passed pitched);
+    w (Cout, Cin, k, k), dz (N, Ho, Wo, Cout), bias (Cout) fp32; workspace a uint8 CUDA tensor (default: allocated)."""
+    for t in (out, w, dz, bias):
+        assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous())
+    x_pitch = 0
+    if x is not None:
+        assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.stride(3) == 1
+        if not x.is_contiguous():
+            N_, H_, W_, _ = x.shape
+            x_pitch = x.stride(2)
+            assert x.stride(1) == W_ * x_pitch and x.stride(0) == H_ * W_ * x_pitch, "x must be a channel slice of an NHWC buffer"
+    if pass_ == 0:
+        (N, H, W, Cin), Cout, k = x.shape, w.shape[0], w.shape[2]
+    elif pass_ == 1:
+        (N, H, W, Cin), Cout, k = out.shape, w.shape[0], w.shape[2]
+    else:
+        (N, H, W, Cin), (Cout, _, k, _) = x.shape, out.shape
+    if workspace is None:
+        need = int(L.lib().yb_conv_tc_workspace_bytes(N, H, W, Cin, Cout, k, stride))
+        workspace = torch.empty(max(need, 256), dtype=torch.uint8, device=out.device)
+    desc = C.create_string_buffer(2048)
+    L.check(L.lib().yb_debug_conv_tf32(pass_, _ptr(x), x_pitch, _ptr(dz), _ptr(w), _ptr(bias), N, H, W, Cin, Cout, k, stride,
+                                       _ptr(out), _ptr(workspace), workspace.numel(), desc, len(desc)))
+    return desc.value.decode()
+
+
 def conv_backward_tc(x, dz, w, stride=1, pad=None, ws=None, stream=None, need_dx=True):
     """yb_conv_backward_data_tc / _weight_tc -> (dx, dw); same tensors as conv_backward."""
     for t in (x, dz, w):
