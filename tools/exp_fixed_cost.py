@@ -1,5 +1,5 @@
 """Experiment: fixed cost of the kernel chain.  Forward time at small batches, with / without PDL
-(YB_DEBUG_NO_PDL=1) and with / without CUDA graph (flags=2).  python tools/exp_fixed_cost.py"""
+(YB_NO_PDL=1) and with / without CUDA graph (flags=2).  python tools/exp_fixed_cost.py"""
 import os
 import sys
 
@@ -28,5 +28,5 @@ for B in (1, 32):
             e.forward(x, out_pred=out)
         b.record()
         torch.cuda.synchronize()
-        print(f"B={B:2d} {label:24s} pdl={'off' if os.environ.get('YB_DEBUG_NO_PDL') else 'on '} forward {a.elapsed_time(b) / 50:.4f} ms", flush=True)
+        print(f"B={B:2d} {label:24s} pdl={'off' if os.environ.get('YB_NO_PDL') else 'on '} forward {a.elapsed_time(b) / 50:.4f} ms", flush=True)
         del e

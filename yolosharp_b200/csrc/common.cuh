@@ -60,16 +60,19 @@ void set_error(const std::string& msg);
     }                                                                                        \
   } while (0)
 
-// ---- programmatic dependent launch for the kernels of the training step ----
+// ---- programmatic dependent launch (PDL) ----
 // A kernel launched through launch_pdl may be scheduled while its predecessor in the stream is still running: its CTAs
 // become resident as the predecessor's retire, run their prologue (parameter loads, barrier setup, descriptor
-// prefetch) and block in pdl_wait() until the predecessor has completed and its writes are visible.  Every such kernel
-// calls pdl_wait() before its first global-memory access and pdl_trigger() right AFTER it: the successor can be scheduled
-// once all CTAs of this kernel have passed their wait, so at most two kernels of the chain are ever in flight (this one
-// finishing, the next one in its prologue).  (Triggering before the wait lets a whole chain of small kernels become
-// resident at once; with that form a seven-kernel loss chain read a scalar before its producer's atomics - not understood,
-// so the conservative order is used everywhere.)  A dependent step of ~800 small kernels otherwise pays a drain + launch +
-// fill at every boundary.
+// prefetch) and block in pdl_wait() until the predecessor has completed and its writes are visible.  Every kernel of the
+// training step calls pdl_wait() before its first global-memory access and pdl_trigger() right AFTER it: the successor
+// can be scheduled once all CTAs of this kernel have passed their wait, so at most two kernels of the chain are ever in
+// flight (this one finishing, the next one in its prologue).  (Triggering before the wait lets a whole chain of small
+// kernels become resident at once; with that form a seven-kernel loss chain read a scalar before its producer's atomics
+// - not understood, so the training step uses the conservative order.)  A dependent step of ~800 small kernels otherwise
+// pays a drain + launch + fill at every boundary.
+// The forward's tensor-core convolutions, fused Bottlenecks and the fp16 SPPF pool (conv_tc.cu, kernels_generic.cu) are
+// launched the same way but trigger before their wait, so that the next layer's prologue (weight prefetch) overlaps
+// this one's tiles.  YB_NO_PDL=1 launches all of these kernels the ordinary way (A/B measurements).
 // Both instructions are no-ops in a kernel launched the ordinary way, so a kernel may be launched either way.
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -147,18 +150,7 @@ struct TcConvPlan;  // opaque: tensor maps + tiling for one conv layer
 TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err);
 void tc_conv_plan_destroy(TcConvPlan* plan);
 std::string tc_conv_plan_describe(const TcConvPlan* plan);  // tiling summary (YB_DEBUG_PLANS)
-// Cross-layer overlap (DESIGN 4.1 "layer chaining"): instead of waiting for the whole previous grid
-// (griddepcontrol.wait) a conv may start a tile as soon as the images it reads are complete in its producer.
-//   done_ctr   this launch's per-image completion counters (rows x N tiles stored), or nullptr
-//   dep_ctr    the producer launch's counters, or nullptr = wait for the previous grid as a whole
-//   dep_expect rows x N tiles the producer stores per image
-struct TcChain {
-  int* done_ctr = nullptr;
-  const int* dep_ctr = nullptr;
-  int dep_expect = 0;
-};
-int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cudaStream_t s, const TcChain* chain = nullptr);
-int tc_conv_rows_per_image(const TcConvPlan* plan);  // rows x N tiles one image contributes to done_ctr
+int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cudaStream_t s);
 bool tc_conv_supported(const ConvParams& p);
 // Fused Bottleneck (DESIGN 4.1): the 3x3 conv `pa` and the 3x3 conv `pb` that reads its output (plus the shortcut
 // `pb` may carry) as one launch; the intermediate stays in shared memory.  Uses both plans' packed weights, so they must

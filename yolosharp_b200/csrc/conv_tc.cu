@@ -70,11 +70,6 @@ struct TcArgs {
   float* pred;
   // exact x / d for x*d < 2^40 as (x * ceil(2^40/d)) >> 40 (runtime integer division costs ~100+ cycles)
   uint64_t m_ntiles, m_tpi, m_tw, m_bw;
-  // layer chaining (TcChain): per-image completion counters instead of a grid-wide dependency
-  int* done_ctr;
-  const int* dep_ctr;
-  int dep_expect;
-  uint64_t m_ohw;  // magic number for / (Ho * Wo) of this conv's output (image of a flattened pixel index)
   int* tile_ctr;   // dynamic tile scheduler: global counter of this launch (nullptr = static round-robin)
   int tile_batch;  // consecutive tiles drawn per atomicAdd (one counter address serves the whole grid)
   long long* dbg;  // optional timeline buffer (tools/exp_timeline.py); nullptr in production
@@ -100,8 +95,9 @@ struct TcConvPlan {
 };
 
 __device__ __forceinline__ int fdiv(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
+// the host side of fdiv: ceil(2^40 / d)
+static uint64_t fdiv_magic(int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); }
 
-__device__ __forceinline__ float silu_fast(float v) { return __fdividef(v, 1.0f + __expf(-v)); }
 // x*sigmoid(x) = h + h*tanh(h), h = x/2: one MUFU op instead of two (ex2 + rcp)
 __device__ __forceinline__ float silu_tanh(float v) {
   const float h = 0.5f * v;
@@ -160,19 +156,6 @@ struct TileDraw {
     if (tile < total) nxt = (int)gridDim.x + atomicAdd(ctr, batch);
   }
 };
-
-// Producer-side dependency wait of the layer chain: poll the producer launch's counter of image `img` until all of
-// its rows are stored (acquire), bounded like every other wait of this kernel.
-__device__ __forceinline__ void dep_wait_image(const int* ctr, int img, int expect) {
-  const long long t0 = clock64();
-  while (true) {
-    int v;
-    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(ctr + img) : "memory");
-    if (v >= expect) break;
-    __nanosleep(100);
-    if (clock64() - t0 > 4000000000ll) __trap();
-  }
-}
 
 // ------------------------------------------------------------------------------------------
 // Main loop of one tile for one consumer warpgroup (its 64 rows of the 128-row tile, all n_tile columns).
@@ -272,46 +255,16 @@ __device__ __forceinline__ void tc_mainloop(const TcArgs& a, float* acc, int wg,
   wg_fence_acc<NT16 * 8>(acc);
 }
 
-// Publish a warp's stored rows per image for the layer chain.  A publish is fence (every lane's stores before the
-// count) + warp barrier + one atomic; the fence costs several hundred cycles, so rows are counted in registers and
-// published only when the warp moves on to another image (tiles arrive in image order) or runs out of tiles.  The
-// 16 rows of a warp may span two images of a flattened tile.
-__device__ __forceinline__ void chain_count(const TcArgs& a, const bool (&valid)[2], const int (&im)[2], int& pend_img,
-                                            int& pend_cnt) {
-  const int lane = threadIdx.x & 31;
-  const bool lead = (lane & 3) == 0;  // one lane of each quad owns the quad's two rows
-  const int cand = valid[0] ? im[0] : (valid[1] ? im[1] : INT_MAX);
-  const int first = __reduce_min_sync(0xffffffffu, cand);
-  if (first == INT_MAX) return;
-  const int nall = __popc(__ballot_sync(0xffffffffu, lead && valid[0])) + __popc(__ballot_sync(0xffffffffu, lead && valid[1]));
-  const int nsame = __popc(__ballot_sync(0xffffffffu, lead && valid[0] && im[0] == first)) +
-                    __popc(__ballot_sync(0xffffffffu, lead && valid[1] && im[1] == first));
-  if (pend_img >= 0 && pend_img != first) {
-    __threadfence();
-    __syncwarp();
-    if (lane == 0) atomicAdd(a.done_ctr + pend_img, pend_cnt);
-    pend_cnt = 0;
-  }
-  pend_img = first;
-  pend_cnt += nsame;
-  if (nall != nsame) {
-    __threadfence();
-    __syncwarp();
-    if (lane == 0) atomicAdd(a.done_ctr + first, pend_cnt);
-    pend_img = first + 1;
-    pend_cnt = nall - nsame;
-  }
-}
-
 // Epilogue of one tile from the accumulator registers: +bias -> SiLU -> +residual -> fp16 into the channel slice of
 // the (concat) output buffer, or the fused Detect tail (DFL box decode / class scores into the prediction tensor).
 template <int NT16>
 __device__ __forceinline__ void tc_epilogue(const TcArgs& a, const float* acc, const float* bias, int n0, int img, int th,
-                                            int tw, int wg, bool (&valid)[2], int (&wo)[2]) {
+                                            int tw, int wg) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t4 = lane & 3;
   size_t pix[2];
-  int ho[2];
+  int ho[2], wo[2];
+  bool valid[2];
 #pragma unroll
   for (int h = 0; h < 2; h++) {
     const int row = wg * 64 + (warp & 3) * 16 + g + 8 * h;
@@ -393,8 +346,7 @@ __device__ __forceinline__ void tc_epilogue(const TcArgs& a, const float* acc, c
       float f0 = acc[4 * J + 2 * h] + b.x, f1 = acc[4 * J + 2 * h + 1] + b.y;
       if (a.act == ACT_SILU) { f0 = silu_tanh(f0); f1 = silu_tanh(f1); }
       if (use_res) {
-        // L2-only load: with layer chaining a neighbouring row of the same 128-byte line may still be unwritten when
-        // this one is read, and a line cached in L1 now would be stale when that row's own tile reads it later
+        // L2-only load: every residual element is read exactly once, so an L1 copy of its line would never be reused
         const unsigned int rb = __ldcg(reinterpret_cast<const unsigned int*>(rrow + c));
         const float2 x = __half22float2(*reinterpret_cast<const __half2*>(&rb));
         f0 += x.x; f1 += x.y;
@@ -435,8 +387,6 @@ __device__ __forceinline__ void tc_fold(const TcArgs& a, const float* acc, const
   constexpr uint32_t ROW16 = KK2 * 2;  // bytes per weight row / 16
   const uint32_t b_hi = wg_desc_hi(a.sbo_b2, a.layout_b2);
   const uint32_t b_lo0 = wg_desc_lo(smemW2), b_slab16 = a.b2_stride >> 4;
-  bool valid[2];
-  int wo[2];
 #pragma unroll
   for (int c0 = 0; c0 < 16 * N2_16; c0 += 16 * F16) {
     float acc2[F16 * 8];
@@ -448,7 +398,7 @@ __device__ __forceinline__ void tc_fold(const TcArgs& a, const float* acc, const
     wg_commit();
     wg_wait<0>();
     wg_fence_acc<F16 * 8>(acc2);
-    tc_epilogue<F16>(a, acc2, bias2 + c0, c0, img, th, tw, wg, valid, wo);
+    tc_epilogue<F16>(a, acc2, bias2 + c0, c0, img, th, tw, wg);
   }
 }
 
@@ -516,9 +466,8 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
       if (N2_16 > 0) bulk_load_1d(smem0 + a.w2_off, a.w2, a.w2_bytes, bfull);  // the folded 1x1's slabs, one copy
     }
   }
-  // activations written by the previous kernel are visible only after this point - unless this launch is chained to
-  // its producer by per-image counters (dep_ctr): then tiles start as soon as their images are complete
-  if (a.dep_ctr == nullptr) asm volatile("griddepcontrol.wait;" ::: "memory");
+  // activations written by the previous kernel are visible only after this point
+  asm volatile("griddepcontrol.wait;" ::: "memory");
 
   const bool dyn = a.tile_ctr != nullptr;
   if (warp == TC_CONSUMER_WARPS) {
@@ -529,26 +478,8 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
       uint32_t pa = 0, pb = 0;
       int li = 0;
       TileDraw td(a.tile_ctr, a.tile_batch, a.total_tiles);
-      int dep_ready = -1;  // last image of the producer known to be complete
       for (; td.tile < a.total_tiles; li++) {
         const int tile = td.tile;
-        if (a.dep_ctr != nullptr) {
-          // images this tile reads: its own image, or for a flattened 1x1 tile the images of its first / last pixel
-          const int mt0 = fdiv(tile, a.m_ntiles);
-          int i0, i1;
-          if (a.imgs == 1 && a.Ho == 1) {
-            const int p0 = mt0 * 128, p1 = min(p0 + 127, a.Wo - 1);
-            i0 = fdiv(p0, a.m_ohw); i1 = fdiv(p1, a.m_ohw);
-          } else {
-            i0 = i1 = fdiv(mt0, a.m_tpi);
-          }
-          if (i1 != dep_ready || i0 != i1) {
-            for (int im = i0; im <= i1; im++)
-              if (im != dep_ready) dep_wait_image(a.dep_ctr, im, a.dep_expect);
-            dep_ready = i1;
-            asm volatile("fence.proxy.async.global;" ::: "memory");  // generic-proxy acquire -> async-proxy (TMA) reads
-          }
-        }
         if (dyn) tq_publish(s_tile, &s_head, li, tile);
         const int mt = fdiv(tile, a.m_ntiles);
         const int nt = tile - mt * a.n_tiles;
@@ -596,7 +527,6 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
     int sa = 0, sb = 0;
     uint32_t pa = 0, pb = 0;
     if (a.b_resident || N2_16 > 0) mbar_wait(bfull, 0);
-    int pend_img = -1, pend_cnt = 0;  // layer chaining: rows stored but not yet published
     const bool dbg_on = a.dbg && blockIdx.x == 0 && threadIdx.x == 0;
     for (int li = 0;; li++) {
       const int tile = dyn ? tq_get(s_tile, &s_head, li) : (int)blockIdx.x + li * (int)gridDim.x;
@@ -615,29 +545,16 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
       const int r = mt - img * tiles_per_img;
       const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
       const int n0 = nt * a.n_tile;
-      if constexpr (N2_16 > 0) {  // one N tile: n0 = 0; never chained
+      if constexpr (N2_16 > 0) {  // one N tile: n0 = 0
         switch (a.BK2) {
           case 64: tc_fold<NT16, N2_16, 4>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, img, th, tw, wg); break;
           case 32: tc_fold<NT16, N2_16, 2>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, img, th, tw, wg); break;
           default: tc_fold<NT16, N2_16, 1>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, img, th, tw, wg); break;
         }
-        if (dbg_on && li < 16) a.dbg[li * 8 + 6] = clock64();
-        continue;
-      }
-      bool valid[2];
-      int wo[2];
-      tc_epilogue<NT16>(a, acc, s_bias + n0, n0, img, th, tw, wg, valid, wo);
-      if (a.done_ctr != nullptr && a.epi_mode == EPI_STORE) {
-        const bool flat1 = a.imgs == 1 && a.Ho == 1;
-        const int im[2] = {flat1 ? fdiv(min(wo[0], a.Wo - 1), a.m_ohw) : img, flat1 ? fdiv(min(wo[1], a.Wo - 1), a.m_ohw) : img};
-        chain_count(a, valid, im, pend_img, pend_cnt);
+      } else {
+        tc_epilogue<NT16>(a, acc, s_bias + n0, n0, img, th, tw, wg);
       }
       if (dbg_on && li < 16) a.dbg[li * 8 + 6] = clock64();
-    }
-    if (pend_img >= 0) {
-      __threadfence();
-      __syncwarp();
-      if (lane == 0) atomicAdd(a.done_ctr + pend_img, pend_cnt);
     }
   }
 }
@@ -690,18 +607,10 @@ bool tc_conv_supported(const ConvParams& p) {
   return true;
 }
 
-// Experiment knob (tools/exp_dual.py): YB_PLAN_SMALL=1 sizes every plan for half an SM (<= 104 KiB of rings) and launches one CTA per SM, so that kernels of TWO concurrent streams (two half-batch
-// engines) are co-resident on every SM and each fills the other's pipeline bubbles.
-static int plan_small() {
-  const char* v = getenv("YB_PLAN_SMALL");
-  return v ? atoi(v) : 0;
-}
-
 static int pick_n_tile(int cout) {
-  const int cap = plan_small() ? 128 : 256;
-  if (cout <= cap) return cout;
+  if (cout <= 256) return cout;
   int best = 16;
-  for (int n = 16; n <= cap; n += 16)
+  for (int n = 16; n <= 256; n += 16)
     if (cout % n == 0) best = n;
   return best;
 }
@@ -743,7 +652,7 @@ static bool tc_size_rings(TcConvPlan* plan, size_t extra, int max_occ) {
     // weight re-fetch per tile
     a.b_resident = (a.n_tiles == 1 && b_all + 3 * (size_t)a.a_stride <= budget) ? 1 : 0;
     // resident weights at one CTA/SM beat re-fetched weights at two CTAs/SM
-    if (occ == 2 && !plan_small() && !small && !a.b_resident && a.n_tiles == 1 && b_all + 3 * (size_t)a.a_stride <= full) continue;
+    if (occ == 2 && !small && !a.b_resident && a.n_tiles == 1 && b_all + 3 * (size_t)a.a_stride <= full) continue;
     if (a.b_resident) {
       a.stages_a = (int)std::min<size_t>(a.mode != TC_TAP ? (a.chunks > 1 ? 8 : 6) : TC_MAX_STAGES, (budget - b_all) / a.a_stride);
       a.stages_b = 0;
@@ -759,13 +668,21 @@ static bool tc_size_rings(TcConvPlan* plan, size_t extra, int max_occ) {
     a.w2_off = (uint32_t)rings;
     plan->smem = rings + extra + 1024;
     const bool fits = a.stages_a >= 2 && (a.b_resident || a.stages_b >= ((occ == 2 && a.mode != TC_TAP) ? 3 : 2)) && rings <= budget;
-    if (fits && (occ == 1 || small || a.stages_a >= 3 || plan_small())) { plan->occ = occ; break; }
+    if (fits && (occ == 1 || small || a.stages_a >= 3)) { plan->occ = occ; break; }
     if (occ == 1) a.stages_a = 0;  // reported below
   }
   plan->small = m_tiles * a.n_tiles <= 2 * num_sms;
   plan->grid = num_sms * plan->occ;
-  if (plan_small() && plan->occ == 2) plan->grid = num_sms;  // the SM's other half belongs to the other stream's kernel
   return !(a.stages_a < 2 || (!a.b_resident && a.stages_b < 2));
+}
+
+// Shared-memory attributes of a conv_tc_kernel instantiation: dynamic limit = ring budget + alignment slack (static smem
+// of the kernel counts against the 227 KiB cap).  false (and *err) on failure.
+static bool tc_kernel_attrs(void (*kernel)(TcArgs), std::string* err) {
+  cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  const cudaError_t ce = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 202 * 1024);
+  if (ce != cudaSuccess && err) *err = std::string("cudaFuncSetAttribute(conv_tc_kernel) failed: ") + cudaGetErrorString(ce);
+  return ce == cudaSuccess;
 }
 
 TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
@@ -912,15 +829,9 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
     return nullptr;
   }
   dispatch_nt16(a.n_tile / 16, [&](auto nt16) { plan->kernel = conv_tc_kernel<decltype(nt16)::value>; });
-  {
-    // dynamic limit = ring budget + alignment slack (static smem of the kernel counts against the 227 KiB cap)
-    cudaFuncSetAttribute(plan->kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaError_t ce = cudaFuncSetAttribute(plan->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 202 * 1024);
-    if (ce != cudaSuccess) {
-      if (err) *err = std::string("cudaFuncSetAttribute(conv_tc_kernel) failed: ") + cudaGetErrorString(ce);
-      delete plan;
-      return nullptr;
-    }
+  if (!tc_kernel_attrs(plan->kernel, err)) {
+    delete plan;
+    return nullptr;
   }
   return plan;
 }
@@ -978,11 +889,9 @@ TcConvPlan* tc_fold_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, std:
     return fail("no fold instantiation for " + std::to_string(a1.n_tile) + " -> " + std::to_string(p2.Cout) + " channels");
   }
   plan->kernel = kernel;
-  cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  const cudaError_t ce = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 202 * 1024);
-  if (ce != cudaSuccess) {
+  if (!tc_kernel_attrs(kernel, err)) {
     delete plan;
-    return fail(std::string("cudaFuncSetAttribute(conv_tc_kernel) failed: ") + cudaGetErrorString(ce));
+    return nullptr;
   }
   return plan;
 }
@@ -1007,16 +916,9 @@ void tc_conv_plan_destroy(TcConvPlan* plan) {
 long long* g_tc_dbg = nullptr;  // set by yb_debug_timeline: next tensor-core conv launches write their timeline here
 int g_tc_dbg_countdown = -1;
 
-int tc_conv_rows_per_image(const TcConvPlan* plan) { return plan->p.Ho * plan->p.Wo * plan->args.n_tiles; }
-
-int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cudaStream_t s, const TcChain* chain) {
+int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cudaStream_t s) {
   TcArgs a = plan->args;
   a.pred = pred;
-  if (chain) {
-    a.done_ctr = chain->done_ctr;
-    a.dep_ctr = chain->dep_ctr;
-    a.dep_expect = chain->dep_expect;
-  }
   a.tile_ctr = tile_ctr;
   a.dbg = nullptr;
   if (g_tc_dbg && g_tc_dbg_countdown >= 0 && g_tc_dbg_countdown-- == 0) a.dbg = g_tc_dbg;
@@ -1034,14 +936,9 @@ int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cu
     a.tiles_h = (p.Ho + a.BH - 1) / a.BH;
   }
   a.total_tiles = a.imgs * a.tiles_w * a.tiles_h * a.n_tiles;
-  auto magic = [](int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); };
-  a.m_ntiles = magic(a.n_tiles); a.m_tpi = magic(a.tiles_w * a.tiles_h); a.m_tw = magic(a.tiles_w); a.m_bw = magic(a.BW);
-  a.m_ohw = magic(p.Ho * p.Wo);
+  a.m_ntiles = fdiv_magic(a.n_tiles); a.m_tpi = fdiv_magic(a.tiles_w * a.tiles_h); a.m_tw = fdiv_magic(a.tiles_w);
+  a.m_bw = fdiv_magic(a.BW);
   int grid = std::min(plan->grid, a.total_tiles);
-  // chained layers: one CTA per SM for the two-CTA plans, so that the other slot of every SM is free for the NEXT
-  // layer's CTA - consecutive layers then run side by side, the later one on the images the earlier one has finished
-  static const int chain_grid1 = getenv("YB_CHAIN_GRID1") ? atoi(getenv("YB_CHAIN_GRID1")) : 1;
-  if (chain && chain_grid1 && plan->occ == 2) grid = std::min(grid, std::max(1, plan->grid / 2));
   // concurrent head branches: a latency-bound layer with ~1 tile per CTA gives up half of its CTAs (each
   // then pipelines 2-3 tiles) so that a sibling branch can occupy the other SMs at the same time
   if (plan->p.share_sms && a.total_tiles <= 4 * plan->grid && a.ksteps * (a.BK >> 4) <= 40)
@@ -1049,18 +946,7 @@ int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cu
   // one atomic per ~quarter of a CTA's share (every atomic of the grid hits the same L2 address, so per-tile draws
   // would serialise the 6400-tile layers)
   a.tile_batch = std::max(1, std::min(8, a.total_tiles / (4 * grid)));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = plan->smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;  // PDL (see griddepcontrol in the kernel)
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  static const bool no_pdl = getenv("YB_DEBUG_NO_PDL") != nullptr;  // experiments only (tools/exp_fixed_cost.py)
-  cfg.numAttrs = no_pdl ? 0 : 1;
-  YB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, plan->kernel, a));
+  YB_CUDA_CHECK(launch_pdl(plan->kernel, dim3(grid), dim3(TC_THREADS), plan->smem, s, a));
   return 0;
 }
 
@@ -1434,10 +1320,7 @@ TcBneckPlan* tc_bneck_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, st
     }
     lim = plan->smem;
   }
-  int dev = 0, num_sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-  plan->grid = num_sms * plan->occ;
+  plan->grid = tc_num_sms() * plan->occ;
   return plan;
 }
 
@@ -1456,22 +1339,11 @@ int tc_bneck_launch(const TcBneckPlan* plan, int B, int* tile_ctr, cudaStream_t 
   a.tiles_w = (a.W + HALO_BW - 1) / HALO_BW;
   a.tiles_h = (a.H + HALO_BH - 1) / HALO_BH;
   a.total_tiles = B * a.tiles_w * a.tiles_h;
-  auto magic = [](int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); };
-  a.m_tpi = magic(a.tiles_w * a.tiles_h); a.m_tw = magic(a.tiles_w);
+  a.m_tpi = fdiv_magic(a.tiles_w * a.tiles_h); a.m_tw = fdiv_magic(a.tiles_w);
   a.tile_ctr = tile_ctr;
   const int grid = std::min(plan->grid, a.total_tiles);
   a.tile_batch = std::max(1, std::min(8, a.total_tiles / (4 * grid)));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = plan->smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;  // PDL (see griddepcontrol in the kernel)
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  YB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, plan->kernel, a));
+  YB_CUDA_CHECK(launch_pdl(plan->kernel, dim3(grid), dim3(TC_THREADS), plan->smem, s, a));
   return 0;
 }
 
@@ -1702,19 +1574,16 @@ int launch_stem_f16(const void* in, int in_dtype, int B, int H, int W, const __h
   a.tiles_w = (a.Wo + ST_TW - 1) / ST_TW;
   a.tiles_h = (a.Ho + ST_TH - 1) / ST_TH;
   a.total_tiles = B * a.tiles_w * a.tiles_h;
-  auto magic = [](int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); };
-  a.m_tpi = magic(a.tiles_w * a.tiles_h); a.m_tw = magic(a.tiles_w);
-  static int num_sms = 0;
+  a.m_tpi = fdiv_magic(a.tiles_w * a.tiles_h); a.m_tw = fdiv_magic(a.tiles_w);
+  static bool attrs_set = false;
   const size_t smem = 1024 + 16 * 1024 + (size_t)a.Cout * 128;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+  if (!attrs_set) {
     YB_CUDA_CHECK(cudaFuncSetAttribute(stem_tc_kernel<YB_U8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     YB_CUDA_CHECK(cudaFuncSetAttribute(stem_tc_kernel<YB_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     YB_CUDA_CHECK(cudaFuncSetAttribute(stem_tc_kernel<YB_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+    attrs_set = true;
   }
-  const int grid = std::min(a.total_tiles, num_sms * 4);
+  const int grid = std::min(a.total_tiles, tc_num_sms() * 4);
   if (in_dtype == YB_U8) stem_tc_kernel<YB_U8><<<grid, ST_THREADS, smem, s>>>(a);
   else if (in_dtype == YB_F16) stem_tc_kernel<YB_F16><<<grid, ST_THREADS, smem, s>>>(a);
   else stem_tc_kernel<YB_F32><<<grid, ST_THREADS, smem, s>>>(a);

@@ -341,10 +341,9 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
   // Two CTAs per SM when there are tiles for them and a CTA fits half an SM (n_tile <= 64: 32 accumulator registers per
   // thread, a ring of >= 3 stages in ~100 KiB): the consumers stall in the epilogue of every tile, and a second CTA fills
   // the other's load -> MMA -> epilogue bubbles, as in conv_tc_kernel.
-  static const bool occ1 = getenv("YB_TF_OCC1") != nullptr;
   const size_t per_stage = (size_t)a.a_stride + a.b_stride;
   int occ = 1;
-  if (!occ1 && a.n_tile <= 64 && (size_t)(100 * 1024) / per_stage >= 3 && a.total_tiles >= 2 * tf_num_sms()) occ = 2;
+  if (a.n_tile <= 64 && (size_t)(100 * 1024) / per_stage >= 3 && a.total_tiles >= 2 * tf_num_sms()) occ = 2;
   a.stages = (int)std::min<size_t>(TF_MAX_STAGES, (size_t)((occ == 2 ? 100 : 190) * 1024) / per_stage);
   if (a.stages < 2) { set_error("tf32 conv: tile does not fit in shared memory"); return YB_ERR_SHAPE; }
   const size_t smem = (size_t)a.stages * (a.a_stride + a.b_stride) + 1024;
@@ -709,8 +708,7 @@ int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W
   a.co_pad = p.co_pad; a.ci_pad = p.ci_pad;
   // 3x3 stride 1: the input tile with its halo is loaded once per pixel tile and the nine taps are row-shifted MMA windows
   // into it (the per-tap form moved 9 x 8 KiB of x per 64 pixels and was bound by L2 -> SM delivery).
-  static const bool no_halo = getenv("YB_WGRAD_NO_HALO") != nullptr;
-  a.halo = (k == 3 && stride == 1 && !no_halo) ? 1 : 0;
+  a.halo = (k == 3 && stride == 1) ? 1 : 0;
   a.xblk = a.halo ? (uint32_t)(((WG_PW + 2) * WG_PH * 128 + 1023) / 1024 * 1024) : (uint32_t)WG_BLK;
   const size_t b_stride = (size_t)p.nb * a.xblk;
   a.b_stages = (int)std::min<size_t>(16, ((size_t)190 * 1024 - (size_t)WG_A_STAGES * 4 * WG_BLK) / b_stride);

@@ -70,7 +70,6 @@ struct OpDesc {
   int lane = 0;        // 0 = main stream; >0 = independent head branch that may run concurrently
   int lane_level = -1; // pyramid level whose feature map a side lane waits for
   int feat_level = -1; // this op completes feats[feat_level] (fork point for the head lanes)
-  int dep_op = -1;     // layer chaining: the op whose per-image completion gates this op's tiles (-1: whole previous grid)
   EpiDecode dec;       // conv: fused Detect-tail epilogue (tensor-core path)
   bool fused = false;  // decode op: its work is done by the producing convs' epilogues
   TcBneckPlan* bneck = nullptr;  // conv: fused Bottleneck that also computes the previous op (its input) in smem
@@ -97,8 +96,6 @@ struct yb_engine {
   char* arena = nullptr;
   size_t arena_bytes = 0;
   int* tile_ctr = nullptr;  // one dynamic-scheduler counter per op, zeroed at the start of every forward
-  int* done_ctr = nullptr;  // layer chaining: [op][image] rows stored (same allocation as tile_ctr, zeroed with it)
-  int chain = 0;  // 0 off, 1 chained, 2 publish counters only (experiments)
   int src_h = 0, src_w = 0;  // size of the caller's (unpadded) images for the forward being enqueued (yb_forward_padded)
   bool finalized = false;
   int esize = 4;  // bytes per activation element
@@ -707,7 +704,7 @@ static int run_ops(yb_engine* e, const void* in, int in_dtype, int B, float* out
   cudaStream_t main_s = s;
   if (only >= 0) input_converted = true;  // single-op timing (yb_time_op): buffers hold the last forward's data
   if (e->tile_ctr)
-    YB_CUDA_CHECK(cudaMemsetAsync(e->tile_ctr, 0, e->ops.size() * (size_t)(1 + e->cfg.max_batch) * sizeof(int), s));
+    YB_CUDA_CHECK(cudaMemsetAsync(e->tile_ctr, 0, e->ops.size() * sizeof(int), s));
   for (size_t i = 0; i < e->ops.size(); i++) {
     if (only >= 0 && (int)i != only) continue;
     OpDesc& op = e->ops[i];
@@ -738,17 +735,7 @@ static int run_ops(yb_engine* e, const void* in, int in_dtype, int B, float* out
         if (op.bneck) {
           rc = tc_bneck_launch(op.bneck, B, e->tile_ctr ? e->tile_ctr + i : nullptr, s);
         } else if (op.use_tc) {
-          TcChain ch;
-          const bool chained = e->chain != 0 && only < 0 && !op.fold;
-          if (chained) {
-            ch.done_ctr = e->done_ctr + i * (size_t)e->cfg.max_batch;
-            if (op.dep_op >= 0) {
-              ch.dep_ctr = e->done_ctr + op.dep_op * (size_t)e->cfg.max_batch;
-              ch.dep_expect = tc_conv_rows_per_image(e->ops[op.dep_op].plan);
-            }
-          }
-          rc = tc_conv_launch(op.fold ? op.fold : op.plan, B, out_pred, e->tile_ctr ? e->tile_ctr + i : nullptr, s,
-                              chained ? &ch : nullptr);
+          rc = tc_conv_launch(op.fold ? op.fold : op.plan, B, out_pred, e->tile_ctr ? e->tile_ctr + i : nullptr, s);
         } else {
           rc = launch_conv_generic<T>(conv_params(e, op, B), s);
         }
@@ -872,13 +859,11 @@ int32_t yb_create(const yb_config* cfg, yb_engine** out) {
   e->arena_bytes = off;
   YB_CUDA_CHECK(cudaMalloc((void**)&e->arena, off));
   YB_CUDA_CHECK(cudaMemset(e->arena, 0, off));
-  YB_CUDA_CHECK(cudaMalloc((void**)&e->tile_ctr, e->ops.size() * (size_t)(1 + cfg->max_batch) * sizeof(int)));
-  e->done_ctr = e->tile_ctr + e->ops.size();
+  YB_CUDA_CHECK(cudaMalloc((void**)&e->tile_ctr, e->ops.size() * sizeof(int)));
   // forward kernels are captured at the highest stream priority: when the caller overlaps post-processing of the
   // previous batch (NMS on another stream) with this forward, freed SMs go to the forward's CTAs first
   int prio_least = 0, prio_greatest = 0;
   YB_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
-  if (getenv("YB_DEBUG_NO_PRIORITY")) prio_greatest = prio_least;  // experiments only
   YB_CUDA_CHECK(cudaStreamCreateWithPriority(&e->capture_stream, cudaStreamNonBlocking, prio_greatest));
   for (int l = 1; l < yb_engine::kLanes; l++) {
     YB_CUDA_CHECK(cudaStreamCreateWithPriority(&e->side[l], cudaStreamNonBlocking, prio_greatest));
@@ -1086,34 +1071,9 @@ int32_t yb_finalize_weights(yb_engine* e) {
     a.absorbed = a.folded = true;
     if (getenv("YB_DEBUG_PLANS")) fprintf(stderr, "[plan] %-30s %s (folds %s)\n", b.name.c_str(), tc_conv_plan_describe(b.fold).c_str(), a.name.c_str());
   }
-  // Layer chaining: inside a lane, a tensor-core conv whose stream predecessor is a tensor-core conv that stores an NHWC
-  // tensor starts its tiles per image, as soon as the predecessor has stored that image (per-image counters), instead
-  // of waiting for the predecessor's whole grid.  Completion per image is monotone along the lane (every op waits for
-  // its predecessor's image before it stores its own), so the predecessor's counter also covers older producers of the
-  // same image (concat slices, shortcut inputs).  Ops after anything else (stem, pool, attention, depthwise convs,
-  // lane forks) keep the grid-wide dependency.
-  e->chain = (allow_tc && getenv("YB_CHAIN")) ? atoi(getenv("YB_CHAIN")) : 0;
-  if (e->chain == 1) {
-    int prev_in_lane[yb_engine::kLanes];
-    for (int l = 0; l < yb_engine::kLanes; l++) prev_in_lane[l] = -1;
-    for (size_t i = 0; i < e->ops.size(); i++) {
-      OpDesc& op = e->ops[i];
-      if ((op.type == OP_DECODE && op.fused) || op.absorbed) continue;  // launches nothing
-      const int lane = (e->cfg.flags & YB_FLAG_NO_CONCURRENCY) ? 0 : op.lane;
-      const int pv = prev_in_lane[lane];
-      // fused Bottlenecks and folds neither wait on nor publish per-image counters: they keep the grid-wide dependency both ways
-      if (op.type == OP_CONV && op.use_tc && !op.bneck && !op.fold && pv >= 0) {
-        const OpDesc& pr = e->ops[pv];
-        if (pr.type == OP_CONV && pr.use_tc && !pr.bneck && !pr.fold && pr.dec.mode == EPI_STORE) op.dep_op = pv;
-      }
-      prev_in_lane[lane] = (int)i;
-    }
-  }
   e->lanes_ok = allow_tc && !(e->cfg.flags & YB_FLAG_NO_CONCURRENCY);
   for (auto& d : e->ops)
     if (d.type == OP_DECODE && !d.fused) e->lanes_ok = false;  // the generic decode kernel joins box+cls lanes
-  for (auto& c : e->ops)
-    if (c.lane > 0 && (c.type == OP_CONV || c.type == OP_DWCONV) && c.type == OP_CONV && !c.use_tc) {}
   e->host.clear();
   e->finalized = true;
   return YB_OK;

@@ -381,17 +381,7 @@ int launch_sppf_pool(const View& in, const View& o5, const View& o9, const View&
       o9.coff % 8 == 0 && o13.coff % 8 == 0 && (size_t)2 * in.H * in.W * 16 <= 48 * 1024) {
     const int HW = in.H * in.W;
     const int threads = std::min(512, (HW + 31) / 32 * 32);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(in.C / 8, B);
-    cfg.blockDim = dim3(threads);
-    cfg.dynamicSmemBytes = (size_t)2 * HW * 16;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    YB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, sppf_pool_h8_kernel, in, o5, o9, o13));
+    YB_CUDA_CHECK(launch_pdl(sppf_pool_h8_kernel, dim3(in.C / 8, B), dim3(threads), (size_t)2 * HW * 16, s, in, o5, o9, o13));
     return 0;
   }
   const size_t smem = (size_t)3 * in.H * in.W * SP_CC * sizeof(float);
@@ -937,22 +927,19 @@ int launch_attention(const View& qkv, const View& out, const View& vout, int B, 
     set_error("attention: key_dim <= 64 and head_dim <= 128 supported");
     return YB_ERR_SHAPE;
   }
-  {
-    static const bool no_tiled = getenv("YB_ATTN_ROWS") != nullptr;  // experiments: the row-streaming kernel below
-    if (kd == ATI_KD && hd == ATI_HD && attention_tiled_32x64_fits(N) && !no_tiled && qkv.pitch % 4 == 0 && qkv.coff % 4 == 0 &&
-        out.pitch % 4 == 0 && out.coff % 4 == 0 && vout.coff % 4 == 0) {
-      const int per = 2 * kd + hd;
-      AttnIO io;
-      const T* base = reinterpret_cast<const T*>(qkv.base) + qkv.coff;
-      io.q = base; io.k = base + kd; io.v = base + 2 * kd;
-      io.in_tok = io.v_tok = qkv.pitch; io.in_img = io.v_img = (long long)N * qkv.pitch;
-      io.q_head = io.k_head = io.v_head = per;
-      io.out = reinterpret_cast<T*>(out.base) + out.coff; io.out_tok = out.pitch; io.out_img = (long long)N * out.pitch;
-      io.vout = reinterpret_cast<T*>(vout.base) + vout.coff;
-      io.row_max = io.row_sum = nullptr;
-      if (vout.pitch != out.pitch) { set_error("attention: out and v copy must share their pitch"); return YB_ERR_SHAPE; }
-      return launch_attention_tiled_32x64<T>(io, B, N, nh, scale, s);
-    }
+  if (kd == ATI_KD && hd == ATI_HD && attention_tiled_32x64_fits(N) && qkv.pitch % 4 == 0 && qkv.coff % 4 == 0 &&
+      out.pitch % 4 == 0 && out.coff % 4 == 0 && vout.coff % 4 == 0) {
+    const int per = 2 * kd + hd;
+    AttnIO io;
+    const T* base = reinterpret_cast<const T*>(qkv.base) + qkv.coff;
+    io.q = base; io.k = base + kd; io.v = base + 2 * kd;
+    io.in_tok = io.v_tok = qkv.pitch; io.in_img = io.v_img = (long long)N * qkv.pitch;
+    io.q_head = io.k_head = io.v_head = per;
+    io.out = reinterpret_cast<T*>(out.base) + out.coff; io.out_tok = out.pitch; io.out_img = (long long)N * out.pitch;
+    io.vout = reinterpret_cast<T*>(vout.base) + vout.coff;
+    io.row_max = io.row_sum = nullptr;
+    if (vout.pitch != out.pitch) { set_error("attention: out and v copy must share their pitch"); return YB_ERR_SHAPE; }
+    return launch_attention_tiled_32x64<T>(io, B, N, nh, scale, s);
   }
   const int nwarps = 8;
   const size_t smem = ((size_t)nwarps * N + 32 * (kd + 1) + 32 * hd) * sizeof(float);

@@ -974,7 +974,7 @@ int attention_backward_f32(const float* q, const float* k, const float* v, const
   YB_CUDA_CHECK(cudaMallocAsync((void**)&stats, (3 * n + (size_t)B * N * nh * hd) * sizeof(float), s));
   float* tmp_out = stats + 3 * n;  // the forward output is recomputed only for its row statistics
   int rc = attention_forward_f32(q, k, v, B, N, nh, kd, hd, scale, tmp_out, stats, stats + n, s);
-  if (!rc && kd == 32 && hd == 64 && ab_fits(N) && getenv("YB_ATTN_BWD_OLD") == nullptr) {
+  if (!rc && kd == 32 && hd == 64 && ab_fits(N)) {
     cudaFuncSetAttribute(attn_bwd_q_32x64, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaFuncSetAttribute(attn_bwd_kv_32x64, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     const dim3 grid((N + AB_T - 1) / AB_T, nh, B);
