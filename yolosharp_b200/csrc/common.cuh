@@ -1,5 +1,6 @@
 // Shared declarations for the yolob200 engine (sm_90a only).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -146,6 +147,13 @@ template <typename T>
 int launch_proto_out(const View& in, float* out, int B, cudaStream_t s);
 
 // ---- conv_tc.cu : wgmma implicit-GEMM conv (fp16 storage, fp32 accumulate) ----
+// Device queries shared by the tensor-core convolutions of conv_tc.cu and conv_tf32.cu, cached after the first call:
+// the driver's cuTensorMapEncodeTiled (nullptr when the entry point is missing) and the SM count of the current device.
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn tmap_encode_fn();
+int sm_count();
 struct TcConvPlan;  // opaque: tensor maps + tiling for one conv layer
 TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err);
 void tc_conv_plan_destroy(TcConvPlan* plan);

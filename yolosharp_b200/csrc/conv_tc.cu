@@ -25,6 +25,9 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
+#include <mutex>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -32,10 +35,41 @@
 
 namespace yb {
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode_fn(std::string* err);
+// exact x / d for x*d < 2^40 as (x * ceil(2^40/d)) >> 40 (runtime integer division costs ~100+ cycles)
+__device__ __forceinline__ int fdiv(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
+// the host side of fdiv: ceil(2^40 / d)
+static uint64_t fdiv_magic(int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); }
+
+// The tiles of one launch: `imgs` images of tiles_h x tiles_w output rectangles, each split into n_tiles N tiles.  Tile
+// index = ((img * tiles_h + th) * tiles_w + tw) * n_tiles + nt; the magic numbers divide by n_tiles, tpi and tiles_w.
+struct TileGrid {
+  int tiles_w, tpi, n_tiles, total;  // tpi = tiles per image
+  uint64_t m_ntiles, m_tpi, m_tw;
+};
+static TileGrid tile_grid(int imgs, int H, int W, int BH, int BW, int n_tiles) {
+  TileGrid g;
+  g.tiles_w = (W + BW - 1) / BW;
+  g.tpi = g.tiles_w * ((H + BH - 1) / BH);
+  g.n_tiles = n_tiles;
+  g.total = imgs * g.tpi * n_tiles;
+  g.m_ntiles = fdiv_magic(n_tiles); g.m_tpi = fdiv_magic(g.tpi); g.m_tw = fdiv_magic(g.tiles_w);
+  return g;
+}
+// Grid of a persistent launch of `total` tiles on at most `max_grid` CTAs, and the tiles per draw from the launch's
+// counter: one atomic per ~quarter of a CTA's share (every atomic of the grid hits the same L2 address, so per-tile
+// draws would serialise the 6400-tile layers)
+static int tc_grid(int max_grid, int total, int* tile_batch) {
+  const int grid = std::min(max_grid, total);
+  *tile_batch = std::max(1, std::min(8, total / (4 * grid)));
+  return grid;
+}
+struct TileCoord { int img, th, tw, nt; };
+__device__ __forceinline__ TileCoord tile_coord(const TileGrid& g, int tile) {
+  const int mt = fdiv(tile, g.m_ntiles);
+  const int img = fdiv(mt, g.m_tpi), r = mt - img * g.tpi;
+  const int th = fdiv(r, g.m_tw);
+  return {img, th, r - th * g.tiles_w, tile - mt * g.n_tiles};
+}
 
 enum TcMode { TC_TAP = 0, TC_HALO = 1, TC_S2P = 2 };
 
@@ -48,7 +82,7 @@ struct TcArgs {
   int out_pitch, out_coff, res_pitch, res_coff;
   int Ho, Wo;            // output extent the tiles cover (flattened for 1x1: Ho = 1, Wo = B*H*W)
   int imgs;              // images the tiles iterate over (1 for flattened 1x1)
-  int tiles_w, tiles_h;  // tiles per image
+  TileGrid tg;
   int BW, BH;
   int n_tile, n_tiles;
   int ksz, stride, pad;
@@ -61,16 +95,14 @@ struct TcArgs {
   uint32_t sbo_a, sbo_b;          // wgmma stride-byte-offset between 8-row groups, >> 4
   uint32_t row_bytes;             // BK * 2
   uint32_t layout_a, layout_b;    // wgmma layout type: 1 = SW128, 2 = SW64, 3 = SW32
-  int total_tiles;
   int b_resident;                 // all weight slabs stay in smem for the CTA's lifetime
   int ksteps;
   // fused head decode (EpiDecode)
   int epi_mode, dA, dCtot, da0, dch0, dWl, dHW;
   float dstride;
   float* pred;
-  // exact x / d for x*d < 2^40 as (x * ceil(2^40/d)) >> 40 (runtime integer division costs ~100+ cycles)
-  uint64_t m_ntiles, m_tpi, m_tw, m_bw;
-  int* tile_ctr;   // dynamic tile scheduler: global counter of this launch (nullptr = static round-robin)
+  uint64_t m_bw;   // fdiv magic of BW
+  int* tile_ctr;   // tile queue: global counter of this launch (nullptr = round-robin order)
   int tile_batch;  // consecutive tiles drawn per atomicAdd (one counter address serves the whole grid)
   long long* dbg;  // optional timeline buffer (tools/exp_timeline.py); nullptr in production
   // folded 1x1 (tc_fold, conv_tc_kernel<NT16, N2_16 > 0>): this conv's activations never leave registers; the next conv, a
@@ -93,10 +125,9 @@ struct TcConvPlan {
   void (*kernel)(TcArgs) = nullptr;  // conv_tc_kernel<n_tile / 16> (<n_tile / 16, fold16> for a folded 1x1)
   int fold16 = 0;                    // folded 1x1 (tc_fold_plan_create): its column pass width / 16
 };
-
-__device__ __forceinline__ int fdiv(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
-// the host side of fdiv: ceil(2^40 / d)
-static uint64_t fdiv_magic(int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); }
+// a plan under construction: every refusal frees its packed weights
+struct TcPlanDestroy { void operator()(TcConvPlan* plan) const { tc_conv_plan_destroy(plan); } };
+using TcPlanPtr = std::unique_ptr<TcConvPlan, TcPlanDestroy>;
 
 // x*sigmoid(x) = h + h*tanh(h), h = x/2: one MUFU op instead of two (ex2 + rcp)
 __device__ __forceinline__ float silu_tanh(float v) {
@@ -109,6 +140,40 @@ __device__ __forceinline__ float silu_tanh(float v) {
 __device__ __forceinline__ uint32_t pack_h2(float x, float y) {
   const __half2 h = __floats2half2_rn(x, y);
   return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+// Accumulator pair acc[0..1] (columns c, c + 1) + bias[c..c + 1] -> SiLU when `silu`: the rounding points every fp16
+// epilogue of this file starts with (fp32 sum + bias, then the activation); the caller adds a residual and rounds to fp16.
+__device__ __forceinline__ float2 bias_act(const float* acc, const float* bias, bool silu) {
+  const float2 b = *reinterpret_cast<const float2*>(bias);
+  float2 f = make_float2(acc[0] + b.x, acc[1] + b.y);
+  if (silu) { f.x = silu_tanh(f.x); f.y = silu_tanh(f.y); }
+  return f;
+}
+
+// Row of accumulator half h of this thread in m64 block `blk` of a tile (wgmma D fragment, tc_ptx.cuh)
+__device__ __forceinline__ int acc_row(int blk, int h) {
+  return blk * 64 + ((threadIdx.x >> 5) & 3) * 16 + ((threadIdx.x & 31) >> 2) + 8 * h;
+}
+
+// Descriptor start shift (16-byte units) of 3x3 tap t inside a staged tile of `pitch`-pixel rows, row16 units per pixel
+__device__ __forceinline__ uint32_t tap_shift(int t, int pitch, uint32_t row16) {
+  return (uint32_t)((t / 3) * pitch + t % 3) * row16;
+}
+
+// Next slot of an n-slot mbarrier ring; the wait parity flips on every wrap
+__device__ __forceinline__ void ring_next(int& s, uint32_t& ph, int n) {
+  if (++s == n) { s = 0; ph ^= 1; }
+}
+
+// Operand rows of 128 / 64 / 32 bytes: the tensor-map swizzle, the wgmma layout type it produces, and (device) the
+// 16-byte piece index XOR of row r under it
+static CUtensorMapSwizzle row_swizzle(int row_bytes) {
+  return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+}
+static uint32_t row_layout(int row_bytes) { return row_bytes == 128 ? 1 : (row_bytes == 64 ? 2 : 3); }
+__device__ __forceinline__ uint32_t row_swizzle_xor(uint32_t r, uint32_t row_bytes) {
+  return row_bytes == 128 ? (r & 7) : (row_bytes == 64 ? ((r >> 1) & 3) : ((r >> 2) & 1));
 }
 
 constexpr int TC_CONSUMERS = 256;                // warps 0-7: two warpgroups, rows 0-63 / 64-127 of every tile
@@ -205,14 +270,14 @@ __device__ __forceinline__ void tc_mainloop(const TcArgs& a, float* acc, int wg,
       mbar_wait(fullA + 8 * sa, pa);
       const uint32_t a_lo = a_lo0 + sa * a_stride16;
       const uint32_t slotA = emptyA + 8 * sa;
-      if (++sa == ra) { sa = 0; pa ^= 1; }
+      ring_next(sa, pa, ra);
 #pragma unroll
       for (int t = 0; t < 9; t++) {
         // row shift of tap t inside the staged input tile (compile-time constants after unrolling):
         //   halo : (kh * (BW+2) + kw) pixel rows
         //   s2p  : pair rows (input pixels 2q, 2q+1), the tile starts at pair w0-1: kw = 0 is the second half
         //          of pair j, kw = 1 / 2 the two halves of pair j+1; kh advances one input row = (BW+1) pairs
-        const uint32_t TAP_HALO = (uint32_t)((t / 3) * (HALO_BW + 2) + (t % 3)) * ROW16;
+        const uint32_t TAP_HALO = tap_shift(t, HALO_BW + 2, ROW16);
         const uint32_t TAP_S2P = (uint32_t)((t / 3) * (HALO_BW + 1) + (t % 3 != 0 ? 1 : 0)) * 2 * ROW16 +
                                  (t % 3 != 1 ? ROW16 : 0);
         const uint32_t tap16 = s2p ? TAP_S2P : TAP_HALO;
@@ -223,7 +288,7 @@ __device__ __forceinline__ void tc_mainloop(const TcArgs& a, float* acc, int wg,
           mbar_wait(fullB + 8 * sb, pb);
           b_lo = b_lo0 + sb * b_stride16;
           relB = emptyB + 8 * sb;
-          if (++sb == rb) { sb = 0; pb ^= 1; }
+          ring_next(sb, pb, rb);
         }
         step(a_lo + tap16, b_lo, t == 8 ? slotA : 0u, relB);  // halo tile free once its 9 taps retired
       }
@@ -233,7 +298,7 @@ __device__ __forceinline__ void tc_mainloop(const TcArgs& a, float* acc, int wg,
       mbar_wait(fullA + 8 * sa, pa);
       const uint32_t a_lo = a_lo0 + sa * a_stride16;
       const uint32_t relA = emptyA + 8 * sa;
-      if (++sa == ra) { sa = 0; pa ^= 1; }
+      ring_next(sa, pa, ra);
       uint32_t b_lo, relB = 0;
       if (resident) {
         b_lo = b_lo0 + ks * b_stride16;
@@ -241,7 +306,7 @@ __device__ __forceinline__ void tc_mainloop(const TcArgs& a, float* acc, int wg,
         mbar_wait(fullB + 8 * sb, pb);
         b_lo = b_lo0 + sb * b_stride16;
         relB = emptyB + 8 * sb;
-        if (++sb == rb) { sb = 0; pb ^= 1; }
+        ring_next(sb, pb, rb);
       }
       step(a_lo, b_lo, relA, relB);
     }
@@ -260,14 +325,13 @@ __device__ __forceinline__ void tc_mainloop(const TcArgs& a, float* acc, int wg,
 template <int NT16>
 __device__ __forceinline__ void tc_epilogue(const TcArgs& a, const float* acc, const float* bias, int n0, int img, int th,
                                             int tw, int wg) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t4 = lane & 3;
+  const int t4 = threadIdx.x & 3;
   size_t pix[2];
   int ho[2], wo[2];
   bool valid[2];
 #pragma unroll
   for (int h = 0; h < 2; h++) {
-    const int row = wg * 64 + (warp & 3) * 16 + g + 8 * h;
+    const int row = acc_row(wg, h);
     const int hl = fdiv(row, a.m_bw), wl = row - hl * a.BW;
     ho[h] = th * a.BH + hl;
     wo[h] = tw * a.BW + wl;
@@ -342,16 +406,14 @@ __device__ __forceinline__ void tc_epilogue(const TcArgs& a, const float* acc, c
 #pragma unroll
     for (int J = 0; J < NT16 * 2; J++) {
       const int c = 8 * J + 2 * t4;
-      const float2 b = *reinterpret_cast<const float2*>(bias + c);
-      float f0 = acc[4 * J + 2 * h] + b.x, f1 = acc[4 * J + 2 * h + 1] + b.y;
-      if (a.act == ACT_SILU) { f0 = silu_tanh(f0); f1 = silu_tanh(f1); }
+      float2 f = bias_act(acc + 4 * J + 2 * h, bias + c, a.act == ACT_SILU);
       if (use_res) {
         // L2-only load: every residual element is read exactly once, so an L1 copy of its line would never be reused
         const unsigned int rb = __ldcg(reinterpret_cast<const unsigned int*>(rrow + c));
         const float2 x = __half22float2(*reinterpret_cast<const __half2*>(&rb));
-        f0 += x.x; f1 += x.y;
+        f.x += x.x; f.y += x.y;
       }
-      *reinterpret_cast<__half2*>(orow + c) = __floats2half2_rn(f0, f1);
+      *reinterpret_cast<__half2*>(orow + c) = __floats2half2_rn(f.x, f.y);
     }
   }
 }
@@ -374,16 +436,12 @@ __device__ __forceinline__ void tc_fold(const TcArgs& a, const float* acc, const
   const int t4 = threadIdx.x & 3;
   uint32_t fr[NT16 * 4];
 #pragma unroll
-  for (int J = 0; J < NT16 * 2; J++) {
-    const int c = 8 * J + 2 * t4;
-    const float2 b = *reinterpret_cast<const float2*>(bias1 + c);
+  for (int J = 0; J < NT16 * 2; J++)
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-      float f0 = acc[4 * J + 2 * h] + b.x, f1 = acc[4 * J + 2 * h + 1] + b.y;
-      if (a.act1 == ACT_SILU) { f0 = silu_tanh(f0); f1 = silu_tanh(f1); }
-      fr[2 * J + h] = pack_h2(f0, f1);  // k step J / 2: fr[4 (J / 2) + 2 (J % 2) + h]
+      const float2 f = bias_act(acc + 4 * J + 2 * h, bias1 + 8 * J + 2 * t4, a.act1 == ACT_SILU);
+      fr[2 * J + h] = pack_h2(f.x, f.y);  // k step J / 2: fr[4 (J / 2) + 2 (J % 2) + h]
     }
-  }
   constexpr uint32_t ROW16 = KK2 * 2;  // bytes per weight row / 16
   const uint32_t b_hi = wg_desc_hi(a.sbo_b2, a.layout_b2);
   const uint32_t b_lo0 = wg_desc_lo(smemW2), b_slab16 = a.b2_stride >> 4;
@@ -433,8 +491,8 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
   const uint32_t bfull = smem_u32(&bars[4 * TC_MAX_STAGES]);
 
   // PDL: let the next kernel of the stream/graph start its prologue while this grid runs; it blocks in
-  // its own griddepcontrol.wait until this grid has completed and flushed.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // its own pdl_wait() until this grid has completed and flushed.
+  pdl_trigger();
 
   if (warp == TC_CONSUMER_WARPS && lane == 0) {
     s_head = 0;
@@ -453,7 +511,6 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
   __syncthreads();
 
   const int taps = a.ksz * a.ksz;
-  const int tiles_per_img = a.tiles_w * a.tiles_h;
 
   if (warp == TC_CONSUMER_WARPS && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmA) : "memory");
@@ -467,9 +524,8 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
     }
   }
   // activations written by the previous kernel are visible only after this point
-  asm volatile("griddepcontrol.wait;" ::: "memory");
+  pdl_wait();
 
-  const bool dyn = a.tile_ctr != nullptr;
   if (warp == TC_CONSUMER_WARPS) {
     // ===================== TMA producer =====================
     if (lane == 0) {
@@ -477,31 +533,26 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
       int sa = 0, sb = 0;
       uint32_t pa = 0, pb = 0;
       int li = 0;
-      TileDraw td(a.tile_ctr, a.tile_batch, a.total_tiles);
-      for (; td.tile < a.total_tiles; li++) {
-        const int tile = td.tile;
-        if (dyn) tq_publish(s_tile, &s_head, li, tile);
-        const int mt = fdiv(tile, a.m_ntiles);
-        const int nt = tile - mt * a.n_tiles;
-        const int img = fdiv(mt, a.m_tpi);
-        const int r = mt - img * tiles_per_img;
-        const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
-        const int wbase = tw * a.BW * a.stride - a.pad;
-        const int hbase = th * a.BH * a.stride - a.pad;
+      TileDraw td(a.tile_ctr, a.tile_batch, a.tg.total);
+      for (; td.tile < a.tg.total; li++) {
+        if (a.tile_ctr) tq_publish(s_tile, &s_head, li, td.tile);
+        const TileCoord tc = tile_coord(a.tg, td.tile);
+        const int wbase = tc.tw * a.BW * a.stride - a.pad;
+        const int hbase = tc.th * a.BH * a.stride - a.pad;
         auto load_b = [&](int t, int ch) {
           mbar_wait(emptyB + 8 * sb, pb ^ 1);
           mbar_arrive_expect_tx(fullB + 8 * sb, a.b_bytes);
-          bulk_load_1d(smemB + sb * a.b_stride, a.wpk + (size_t)((nt * taps + t) * a.chunks + ch) * a.b_stride, a.b_bytes,
+          bulk_load_1d(smemB + sb * a.b_stride, a.wpk + (size_t)((tc.nt * taps + t) * a.chunks + ch) * a.b_stride, a.b_bytes,
                        fullB + 8 * sb);
-          if (++sb == rb) { sb = 0; pb ^= 1; }
+          ring_next(sb, pb, rb);
         };
         if (a.mode != TC_TAP) {
           for (int ch = 0; ch < a.chunks; ch++) {
             mbar_wait(emptyA + 8 * sa, pa ^ 1);
             mbar_arrive_expect_tx(fullA + 8 * sa, a.a_bytes);
-            tma_load_4d(smemA + sa * a.a_stride, &a.tmA, fullA + 8 * sa, ch * a.BK, a.mode == TC_S2P ? tw * a.BW - 1 : wbase,
-                        hbase, img);
-            if (++sa == ra) { sa = 0; pa ^= 1; }
+            tma_load_4d(smemA + sa * a.a_stride, &a.tmA, fullA + 8 * sa, ch * a.BK, a.mode == TC_S2P ? tc.tw * a.BW - 1 : wbase,
+                        hbase, tc.img);
+            ring_next(sa, pa, ra);
             if (!a.b_resident)
               for (int t = 0; t < taps; t++) load_b(t, ch);
           }
@@ -511,15 +562,15 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
             for (int ch = 0; ch < a.chunks; ch++) {
               mbar_wait(emptyA + 8 * sa, pa ^ 1);
               mbar_arrive_expect_tx(fullA + 8 * sa, a.a_bytes);
-              tma_load_4d(smemA + sa * a.a_stride, &a.tmA, fullA + 8 * sa, ch * a.BK, wbase + kw, hbase + kh, img);
-              if (++sa == ra) { sa = 0; pa ^= 1; }
+              tma_load_4d(smemA + sa * a.a_stride, &a.tmA, fullA + 8 * sa, ch * a.BK, wbase + kw, hbase + kh, tc.img);
+              ring_next(sa, pa, ra);
               if (!a.b_resident) load_b(t, ch);
             }
           }
         }
         td.advance();
       }
-      if (dyn) tq_publish(s_tile, &s_head, li, -1);  // end mark
+      if (a.tile_ctr) tq_publish(s_tile, &s_head, li, -1);  // end mark
     }
   } else {
     // ===================== consumers: wgmma main loop + epilogue =====================
@@ -529,8 +580,10 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
     if (a.b_resident || N2_16 > 0) mbar_wait(bfull, 0);
     const bool dbg_on = a.dbg && blockIdx.x == 0 && threadIdx.x == 0;
     for (int li = 0;; li++) {
-      const int tile = dyn ? tq_get(s_tile, &s_head, li) : (int)blockIdx.x + li * (int)gridDim.x;
-      if (tile < 0 || tile >= a.total_tiles) break;
+      // without a counter (round-robin order) the consumers compute the producer's sequence themselves; sending it
+      // through the queue as well costs up to 4 registers and a spill in some instantiations (ptxas -v, CUDA 12.9)
+      const int tile = a.tile_ctr ? tq_get(s_tile, &s_head, li) : (int)blockIdx.x + li * (int)gridDim.x;
+      if (tile < 0 || tile >= a.tg.total) break;
       if (dbg_on && li < 16) a.dbg[li * 8 + 0] = clock64();
       float acc[NT16 * 8];
       switch (a.BK) {
@@ -539,20 +592,16 @@ __global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(NT16, N2_16)) conv_
         default: tc_mainloop<NT16, 1>(a, acc, wg, smemA, smemB, fullA, emptyA, fullB, emptyB, sa, pa, sb, pb); break;
       }
       if (dbg_on && li < 16) a.dbg[li * 8 + 3] = clock64();
-      const int mt = fdiv(tile, a.m_ntiles);
-      const int nt = tile - mt * a.n_tiles;
-      const int img = fdiv(mt, a.m_tpi);
-      const int r = mt - img * tiles_per_img;
-      const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
-      const int n0 = nt * a.n_tile;
+      const TileCoord tc = tile_coord(a.tg, tile);
       if constexpr (N2_16 > 0) {  // one N tile: n0 = 0
         switch (a.BK2) {
-          case 64: tc_fold<NT16, N2_16, 4>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, img, th, tw, wg); break;
-          case 32: tc_fold<NT16, N2_16, 2>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, img, th, tw, wg); break;
-          default: tc_fold<NT16, N2_16, 1>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, img, th, tw, wg); break;
+          case 64: tc_fold<NT16, N2_16, 4>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, tc.img, tc.th, tc.tw, wg); break;
+          case 32: tc_fold<NT16, N2_16, 2>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, tc.img, tc.th, tc.tw, wg); break;
+          default: tc_fold<NT16, N2_16, 1>(a, acc, s_bias, s_bias + TC_FOLD_BIAS, smem0 + a.w2_off, tc.img, tc.th, tc.tw, wg); break;
         }
       } else {
-        tc_epilogue<NT16>(a, acc, s_bias + n0, n0, img, th, tw, wg);
+        const int n0 = tc.nt * a.n_tile;
+        tc_epilogue<NT16>(a, acc, s_bias + n0, n0, tc.img, tc.th, tc.tw, wg);
       }
       if (dbg_on && li < 16) a.dbg[li * 8 + 6] = clock64();
     }
@@ -576,7 +625,7 @@ __global__ void pack_weights_kernel(const __half* __restrict__ w, uint8_t* __res
   const size_t K = (size_t)taps * Cin;
   if (ch * BK + c * 8 >= Cin) return;  // ragged last slab: stays zero
   const int4 v = *reinterpret_cast<const int4*>(w + (size_t)(nt * n_tile + r) * K + (size_t)t * Cin + ch * BK + c * 8);
-  const int sw = BK == 64 ? (r & 7) : (BK == 32 ? ((r >> 1) & 3) : ((r >> 2) & 1));
+  const uint32_t sw = row_swizzle_xor((uint32_t)r, (uint32_t)BK * 2);
   uint8_t* slab = out + (size_t)((nt * taps + t) * chunks + ch) * b_stride;
   *reinterpret_cast<int4*>(slab + (size_t)r * BK * 2 + ((c ^ sw) << 4)) = v;
 }
@@ -584,19 +633,56 @@ __global__ void pack_weights_kernel(const __half* __restrict__ w, uint8_t* __res
 // ------------------------------------------------------------------------------------------
 // Host side: tiling choice + tensor maps
 // ------------------------------------------------------------------------------------------
-static EncodeTiledFn get_encode_fn(std::string* err) {
+EncodeTiledFn tmap_encode_fn() {
   static EncodeTiledFn fn = nullptr;
   if (fn) return fn;
   void* p = nullptr;
   cudaDriverEntryPointQueryResult qres;
-  cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres);
-  if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || !p) {
-    if (err) *err = "cuTensorMapEncodeTiled entry point not found";
+  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess ||
+      qres != cudaDriverEntryPointSuccess || !p) {
     cudaGetLastError();
     return nullptr;
   }
   fn = (EncodeTiledFn)p;
   return fn;
+}
+
+int sm_count() {
+  static int num_sms = 0;
+  if (!num_sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return num_sms;
+}
+
+// 4-D tensor map {C, W, H, N} of an fp16 NHWC buffer whose pixels are `pitch` channels apart, starting at channel coff
+static CUresult tmap_nhwc(CUtensorMap* map, void* base, int coff, int C, int W, int H, int N, int pitch, const cuuint32_t* box,
+                          const cuuint32_t* estr, CUtensorMapSwizzle swz) {
+  const EncodeTiledFn encode = tmap_encode_fn();
+  if (!encode) return CUDA_ERROR_NOT_FOUND;
+  const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  const cuuint64_t gstr[3] = {(cuuint64_t)pitch * 2, (cuuint64_t)pitch * 2 * W, (cuuint64_t)pitch * 2 * W * H};
+  return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, static_cast<__half*>(base) + coff, gdim, gstr, box, estr,
+                CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+// Dynamic shared-memory limit of a kernel for a launch of `smem` bytes (and, for the persistent ring kernels, the
+// largest carveout).  Plans of different shapes share an instantiation: its limit (per device) only ever grows to the
+// largest plan made so far, so a smaller plan created later cannot make an earlier one's launch fail.
+static cudaError_t smem_limit(const void* kernel, size_t smem, bool max_carveout) {
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, size_t> limit;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (max_carveout) cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& lim = limit[{dev, kernel}];
+  if (smem <= lim) return cudaSuccess;
+  const cudaError_t ce = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (ce == cudaSuccess) lim = smem;
+  return ce;
 }
 
 bool tc_conv_supported(const ConvParams& p) {
@@ -615,16 +701,6 @@ static int pick_n_tile(int cout) {
   return best;
 }
 
-static int tc_num_sms() {
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return num_sms;
-}
-
 // Operand rings of a plan: stages, resident weights, CTAs per SM and dynamic shared memory.  `extra` bytes of the budget
 // hold the resident weights of a folded 1x1 (tc_fold_plan_create), placed after the rings at args.w2_off.  Returns
 // false when the tile does not fit.
@@ -635,7 +711,7 @@ static int tc_num_sms() {
 static bool tc_size_rings(TcConvPlan* plan, size_t extra, int max_occ) {
   TcArgs& a = plan->args;
   const ConvParams& p = plan->p;
-  const int num_sms = tc_num_sms();
+  const int num_sms = sm_count();
   const size_t b_all = (size_t)a.ksteps * a.b_stride;
   const int m_tiles = plan->flat ? (p.B * p.Ho * p.Wo + 127) / 128
                                  : p.B * ((p.Wo + a.BW - 1) / a.BW) * ((p.Ho + a.BH - 1) / a.BH);
@@ -676,19 +752,15 @@ static bool tc_size_rings(TcConvPlan* plan, size_t extra, int max_occ) {
   return !(a.stages_a < 2 || (!a.b_resident && a.stages_b < 2));
 }
 
-// Shared-memory attributes of a conv_tc_kernel instantiation: dynamic limit = ring budget + alignment slack (static smem
-// of the kernel counts against the 227 KiB cap).  false (and *err) on failure.
-static bool tc_kernel_attrs(void (*kernel)(TcArgs), std::string* err) {
-  cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  const cudaError_t ce = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 202 * 1024);
+// Shared-memory limit of a conv_tc_kernel plan's instantiation (smem_limit).  false (and *err) on failure.
+static bool tc_kernel_attrs(const TcConvPlan* plan, std::string* err) {
+  const cudaError_t ce = smem_limit((const void*)plan->kernel, plan->smem, true);
   if (ce != cudaSuccess && err) *err = std::string("cudaFuncSetAttribute(conv_tc_kernel) failed: ") + cudaGetErrorString(ce);
   return ce == cudaSuccess;
 }
 
 TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
-  EncodeTiledFn encode = get_encode_fn(err);
-  if (!encode) return nullptr;
-  TcConvPlan* plan = new TcConvPlan();
+  TcPlanPtr plan(new TcConvPlan());
   plan->p = p;
   TcArgs& a = plan->args;
   memset(&a, 0, sizeof(a));
@@ -712,75 +784,52 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
   a.act = p.act;
   a.n_tile = pick_n_tile(p.Cout);
   a.n_tiles = p.Cout / a.n_tile;
-  const CUtensorMapSwizzle swz = a.BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                            : (a.BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-  a.layout_a = a.layout_b = a.BK == 64 ? 1 : (a.BK == 32 ? 2 : 3);
   a.row_bytes = a.BK * 2;
+  a.layout_a = a.layout_b = row_layout(a.row_bytes);
   a.sbo_a = a.sbo_b = (8 * a.row_bytes) >> 4;
-  // stride-2 3x3, pair rows: two horizontally adjacent pixels (input columns 2q, 2q+1) are contiguous in a
-  // whole-buffer NHWC view, so the tensor map declares them as ONE row of 2*Cin channels with the swizzle of
-  // that width.  One dense box of (2BH+1) input rows x (BW+1) pairs then serves all 9 taps as row / K-slice
-  // shifts (see tc_mainloop); the left / top zero padding is TMA out-of-bounds fill of pair -1 / row -1.
-  // (A strided box per tap moves 9 x 128 rows of Cin*2 bytes per tile and is bound by the TMA row rate.)
-  CUtensorMapSwizzle swz_a = swz;
-  if (a.mode == TC_S2P) {
-    swz_a = a.BK == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    a.layout_a = a.BK == 32 ? 1 : 2;
-  }
 
+  // the input as a 4-D NHWC tensor map {C, W, H, N}: the view itself, or re-shaped below
   plan->flat = (p.k == 1 && p.stride == 1);
-  const size_t esz = 2;
-  cuuint64_t gdim[4], gstr[3];
-  cuuint32_t box[4], estr[4];
-  char* base = reinterpret_cast<char*>(p.in.base) + (size_t)p.in.coff * esz;
+  int mC = p.Cin, mW = p.in.W, mH = p.in.H, mN = p.B, m_pitch = p.in.pitch, m_row_bytes = a.row_bytes;
+  cuuint32_t box[4] = {(cuuint32_t)a.BK, 0, 0, 1}, estr[4] = {1, 1, 1, 1};
   if (plan->flat) {
     // all pixels of the batch form one dimension: tiles of 128 consecutive pixels
-    const cuuint64_t npix = (cuuint64_t)p.B * p.in.H * p.in.W;
-    gdim[0] = p.Cin; gdim[1] = npix; gdim[2] = 1; gdim[3] = 1;
-    gstr[0] = (cuuint64_t)p.in.pitch * esz; gstr[1] = gstr[0] * npix; gstr[2] = gstr[1];
+    mW = p.B * p.in.H * p.in.W; mH = mN = 1;
     a.BW = 128; a.BH = 1;
-    box[0] = a.BK; box[1] = 128; box[2] = 1; box[3] = 1;
-    estr[0] = estr[1] = estr[2] = estr[3] = 1;
+    box[1] = 128; box[2] = 1;
+  } else if (a.mode == TC_HALO) {
+    // 8 x 16 output pixels; one TMA box carries the 10 x 18 input halo of a channel slab
+    a.BW = HALO_BW; a.BH = HALO_BH;
+    a.sbo_a = ((a.BW + 2) * a.row_bytes) >> 4;
+    box[1] = a.BW + 2; box[2] = a.BH + 2;
+  } else if (a.mode == TC_S2P) {
+    // stride-2 3x3, pair rows: two horizontally adjacent pixels (input columns 2q, 2q+1) are contiguous in a
+    // whole-buffer NHWC view, so the tensor map declares them as ONE row of 2*Cin channels with the swizzle of
+    // that width.  One dense box of (2BH+1) input rows x (BW+1) pairs then serves all 9 taps as row / K-slice
+    // shifts (see tc_mainloop); the left / top zero padding is TMA out-of-bounds fill of pair -1 / row -1.
+    // (A strided box per tap moves 9 x 128 rows of Cin*2 bytes per tile and is bound by the TMA row rate.)
+    // 8 x 16 output pixels from 9 pairs x 33 input rows; consecutive output rows are two input rows = 18 pair rows apart
+    a.BW = HALO_BW; a.BH = HALO_BH;
+    a.sbo_a = (2 * (a.BW + 1) * 2 * a.row_bytes) >> 4;
+    mC = 2 * p.Cin; mW = p.in.W / 2; m_pitch = 2 * p.in.pitch; m_row_bytes = 2 * a.row_bytes;
+    a.layout_a = row_layout(m_row_bytes);
+    box[0] = 2 * a.BK; box[1] = a.BW + 1; box[2] = 2 * a.BH + 1;
   } else {
-    gdim[0] = p.Cin; gdim[1] = p.in.W; gdim[2] = p.in.H; gdim[3] = p.B;
-    gstr[0] = (cuuint64_t)p.in.pitch * esz;
-    gstr[1] = gstr[0] * p.in.W;
-    gstr[2] = gstr[1] * p.in.H;
-    if (a.mode == TC_HALO) {
-      // 8 x 16 output pixels; one TMA box carries the 10 x 18 input halo of a channel slab
-      a.BW = HALO_BW; a.BH = HALO_BH;
-      a.sbo_a = ((a.BW + 2) * a.row_bytes) >> 4;
-      box[0] = a.BK; box[1] = a.BW + 2; box[2] = a.BH + 2; box[3] = 1;
-      estr[0] = estr[1] = estr[2] = estr[3] = 1;
-    } else if (a.mode == TC_S2P) {
-      // 8 x 16 output pixels from 9 pairs x 33 input rows; consecutive output rows are two input rows =
-      // 18 pair rows apart
-      a.BW = HALO_BW; a.BH = HALO_BH;
-      a.sbo_a = (2 * (a.BW + 1) * 2 * a.row_bytes) >> 4;
-      gdim[0] = 2 * p.Cin; gdim[1] = p.in.W / 2;
-      gstr[0] = (cuuint64_t)2 * p.in.pitch * esz;
-      box[0] = 2 * a.BK; box[1] = a.BW + 1; box[2] = 2 * a.BH + 1; box[3] = 1;
-      estr[0] = estr[1] = estr[2] = estr[3] = 1;
-    } else {
-      // choose the output rectangle BW x BH (<= 128 rows) with the least padding waste
-      double best = -1;
-      for (int bw = 1; bw <= std::min(p.Wo, 128); bw++) {
-        const int bh = std::min(p.Ho, 128 / bw);
-        if (bw * p.stride > 256 || bh * p.stride > 256) continue;
-        const double tiles = (double)((p.Wo + bw - 1) / bw) * ((p.Ho + bh - 1) / bh);
-        const double eff = (double)p.Wo * p.Ho / (tiles * 128.0);
-        if (eff > best + 1e-9 || (eff > best - 1e-9 && bw > a.BW)) { best = eff; a.BW = bw; a.BH = bh; }
-      }
-      box[0] = a.BK; box[1] = a.BW * p.stride; box[2] = a.BH * p.stride; box[3] = 1;
-      estr[0] = 1; estr[1] = p.stride; estr[2] = p.stride; estr[3] = 1;
+    // choose the output rectangle BW x BH (<= 128 rows) with the least padding waste
+    double best = -1;
+    for (int bw = 1; bw <= std::min(p.Wo, 128); bw++) {
+      const int bh = std::min(p.Ho, 128 / bw);
+      if (bw * p.stride > 256 || bh * p.stride > 256) continue;
+      const double tiles = (double)((p.Wo + bw - 1) / bw) * ((p.Ho + bh - 1) / bh);
+      const double eff = (double)p.Wo * p.Ho / (tiles * 128.0);
+      if (eff > best + 1e-9 || (eff > best - 1e-9 && bw > a.BW)) { best = eff; a.BW = bw; a.BH = bh; }
     }
+    box[1] = a.BW * p.stride; box[2] = a.BH * p.stride;
+    estr[1] = estr[2] = p.stride;
   }
-  CUresult cr = encode(&a.tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, gdim, gstr, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, swz_a, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUresult cr = tmap_nhwc(&a.tmA, p.in.base, p.in.coff, mC, mW, mH, mN, m_pitch, box, estr, row_swizzle(m_row_bytes));
   if (cr != CUDA_SUCCESS) {
     if (err) *err = "cuTensorMapEncodeTiled(A) failed with code " + std::to_string((int)cr);
-    delete plan;
     return nullptr;
   }
   const int a_rows = a.mode == TC_HALO ? (a.BW + 2) * (a.BH + 2)
@@ -798,7 +847,7 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
     if (cudaMalloc(&plan->wpk, total) != cudaSuccess) {
       if (err) *err = "cudaMalloc(packed weights) failed";
       cudaGetLastError();
-      delete plan;
+      plan->wpk = nullptr;
       return nullptr;
     }
     cudaMemset(plan->wpk, 0, total);
@@ -809,15 +858,12 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
                                                                     a.b_stride, pieces);
     if (cudaDeviceSynchronize() != cudaSuccess) {
       if (err) *err = std::string("pack_weights_kernel failed: ") + cudaGetErrorString(cudaGetLastError());
-      cudaFree(plan->wpk);
-      delete plan;
       return nullptr;
     }
     a.wpk = plan->wpk;
   }
-  if (!tc_size_rings(plan, 0, tc_ctas_per_sm(a.n_tile / 16, 0))) {
+  if (!tc_size_rings(plan.get(), 0, tc_ctas_per_sm(a.n_tile / 16, 0))) {
     if (err) *err = "tile does not fit in shared memory";
-    delete plan;
     return nullptr;
   }
   a.epi_mode = p.dec.mode;
@@ -825,15 +871,11 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
   a.dstride = p.dec.stride;
   if (a.epi_mode != EPI_STORE && !(plan->flat && a.n_tiles == 1 && (a.epi_mode != EPI_DFL_BOX || a.n_tile == 64))) {
     if (err) *err = "fused decode epilogue needs a flattened 1x1 conv with a single N tile";
-    delete plan;
     return nullptr;
   }
   dispatch_nt16(a.n_tile / 16, [&](auto nt16) { plan->kernel = conv_tc_kernel<decltype(nt16)::value>; });
-  if (!tc_kernel_attrs(plan->kernel, err)) {
-    delete plan;
-    return nullptr;
-  }
-  return plan;
+  if (!tc_kernel_attrs(plan.get(), err)) return nullptr;
+  return plan.release();
 }
 
 // The fold instantiations, as (this conv's n_tile, the 1x1's Cout) / 16: the pairs of the YOLOv8 / YOLOv11 detection
@@ -865,7 +907,7 @@ TcConvPlan* tc_fold_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, std:
   const int nt16 = a1.n_tile / 16, n2_16 = p2.Cout / 16;
   // column passes of at most 80: the second accumulator stays within the register budget of the producer's tile
   const int f16 = tc_fold_pass16(n2_16);
-  TcConvPlan* plan = new TcConvPlan(*pa);
+  TcPlanPtr plan(new TcConvPlan(*pa));
   plan->wpk = nullptr;  // both slab sets belong to the two conv plans
   plan->fold16 = f16;
   TcArgs& a = plan->args;
@@ -879,21 +921,13 @@ TcConvPlan* tc_fold_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, std:
   a.act = a2.act;
   a.epi_mode = a2.epi_mode;
   a.dA = a2.dA; a.dCtot = a2.dCtot; a.da0 = a2.da0; a.dch0 = a2.dch0; a.dWl = a2.dWl; a.dHW = a2.dHW; a.dstride = a2.dstride;
-  if (!tc_size_rings(plan, a.w2_bytes, tc_ctas_per_sm(nt16, n2_16))) {
-    delete plan;
+  if (!tc_size_rings(plan.get(), a.w2_bytes, tc_ctas_per_sm(nt16, n2_16)))
     return fail("the producer's rings and the 1x1's " + std::to_string(a.w2_bytes / 1024) + " KiB of weights do not fit in shared memory");
-  }
-  void (*kernel)(TcArgs) = tc_fold_kernel(nt16, n2_16);
-  if (!kernel || (a2.epi_mode == EPI_DFL_BOX && f16 != 4)) {
-    delete plan;
+  plan->kernel = tc_fold_kernel(nt16, n2_16);
+  if (!plan->kernel || (a2.epi_mode == EPI_DFL_BOX && f16 != 4))
     return fail("no fold instantiation for " + std::to_string(a1.n_tile) + " -> " + std::to_string(p2.Cout) + " channels");
-  }
-  plan->kernel = kernel;
-  if (!tc_kernel_attrs(kernel, err)) {
-    delete plan;
-    return nullptr;
-  }
-  return plan;
+  if (!tc_kernel_attrs(plan.get(), err)) return nullptr;
+  return plan.release();
 }
 
 std::string tc_conv_plan_describe(const TcConvPlan* plan) {
@@ -923,29 +957,22 @@ int tc_conv_launch(const TcConvPlan* plan, int B, float* pred, int* tile_ctr, cu
   a.dbg = nullptr;
   if (g_tc_dbg && g_tc_dbg_countdown >= 0 && g_tc_dbg_countdown-- == 0) a.dbg = g_tc_dbg;
   const ConvParams& p = plan->p;
-  if (plan->flat) {
+  if (plan->flat) {  // 128-pixel tiles of the flattened batch (BW = 128, BH = 1)
     a.imgs = 1;
     a.Ho = 1;
     a.Wo = B * p.Ho * p.Wo;
-    a.tiles_h = 1;
-    a.tiles_w = (a.Wo + 127) / 128;
   } else {
     a.imgs = B;
     a.Ho = p.Ho; a.Wo = p.Wo;
-    a.tiles_w = (p.Wo + a.BW - 1) / a.BW;
-    a.tiles_h = (p.Ho + a.BH - 1) / a.BH;
   }
-  a.total_tiles = a.imgs * a.tiles_w * a.tiles_h * a.n_tiles;
-  a.m_ntiles = fdiv_magic(a.n_tiles); a.m_tpi = fdiv_magic(a.tiles_w * a.tiles_h); a.m_tw = fdiv_magic(a.tiles_w);
+  a.tg = tile_grid(a.imgs, a.Ho, a.Wo, a.BH, a.BW, a.n_tiles);
   a.m_bw = fdiv_magic(a.BW);
-  int grid = std::min(plan->grid, a.total_tiles);
+  int max_grid = plan->grid;
   // concurrent head branches: a latency-bound layer with ~1 tile per CTA gives up half of its CTAs (each
   // then pipelines 2-3 tiles) so that a sibling branch can occupy the other SMs at the same time
-  if (plan->p.share_sms && a.total_tiles <= 4 * plan->grid && a.ksteps * (a.BK >> 4) <= 40)
-    grid = std::max(1, std::min(grid, (a.total_tiles + 2) / 3));
-  // one atomic per ~quarter of a CTA's share (every atomic of the grid hits the same L2 address, so per-tile draws
-  // would serialise the 6400-tile layers)
-  a.tile_batch = std::max(1, std::min(8, a.total_tiles / (4 * grid)));
+  if (plan->p.share_sms && a.tg.total <= 4 * plan->grid && a.ksteps * (a.BK >> 4) <= 40)
+    max_grid = std::min(max_grid, (a.tg.total + 2) / 3);
+  const int grid = tc_grid(max_grid, a.tg.total, &a.tile_batch);
   YB_CUDA_CHECK(launch_pdl(plan->kernel, dim3(grid), dim3(TC_THREADS), plan->smem, s, a));
   return 0;
 }
@@ -980,8 +1007,8 @@ struct BnArgs {
   __half* out;
   int out_pitch, out_coff;
   int shortcut;
-  int H, W, tiles_w, tiles_h, total_tiles;
-  uint64_t m_tpi, m_tw;
+  int H, W;
+  TileGrid tg;
   int cmid, cout;
   int BK1, chunks1, BK2, chunks2;
   uint32_t layout1, layout2;          // wgmma layout types of the BK1 / BK2 rows
@@ -1002,8 +1029,7 @@ struct TcBneckPlan {
 
 // byte offset of (row r, byte b) in a slab of `rb`-byte swizzled rows whose base is 1 KiB aligned (pack_weights_kernel)
 __device__ __forceinline__ uint32_t sw_off(uint32_t r, uint32_t b, uint32_t rb) {
-  const uint32_t sw = rb == 128 ? (r & 7) : (rb == 64 ? ((r >> 1) & 3) : ((r >> 2) & 1));
-  return r * rb + ((((b >> 4) ^ sw)) << 4) + (b & 15);
+  return r * rb + (((b >> 4) ^ row_swizzle_xor(r, rb)) << 4) + (b & 15);
 }
 
 // stage 1 of one warpgroup: MMA rows 128 wg .. 128 wg + 127 as two 64-row accumulators, one commit group per tile
@@ -1017,8 +1043,8 @@ __device__ __forceinline__ void bn_stage1(const BnArgs& a, float (&acc)[2][NM16 
     const uint32_t a_lo = wg_desc_lo(xslot + ch * a.x_stride) + (uint32_t)wg * 128 * RB16;
 #pragma unroll
     for (int t = 0; t < 9; t++) {
-      const uint32_t tap = (uint32_t)((t / 3) * BN_PITCH + t % 3) * RB16;
-      const uint32_t b_lo = wg_desc_lo(w1 + (t * a.chunks1 + ch) * a.b1_stride);
+      const uint32_t tap = tap_shift(t, BN_PITCH, RB16);
+      const uint32_t b_lo = wg_desc_lo(w1 +(t * a.chunks1 + ch) * a.b1_stride);
 #pragma unroll
       for (int k = 0; k < KK; k++) {
 #pragma unroll
@@ -1044,8 +1070,8 @@ __device__ __forceinline__ void bn_stage2(const BnArgs& a, float* acc, uint32_t 
     const uint32_t a_lo = wg_desc_lo(tbase + ch * a.t_stride) + (uint32_t)wg * 8 * BN_PITCH * RB16;
 #pragma unroll
     for (int t = 0; t < 9; t++) {
-      const uint32_t tap = (uint32_t)((t / 3) * BN_PITCH + t % 3) * RB16;
-      const uint32_t b_lo = wg_desc_lo(w2 + (t * a.chunks2 + ch) * a.b2_stride);
+      const uint32_t tap = tap_shift(t, BN_PITCH, RB16);
+      const uint32_t b_lo = wg_desc_lo(w2 +(t * a.chunks2 + ch) * a.b2_stride);
 #pragma unroll
       for (int k = 0; k < KK; k++) {
         wg_mma_n<NO16, false>(acc, a_lo + tap + 2 * k, a_hi, b_lo + 2 * k, b_hi, RB16, scale);
@@ -1092,7 +1118,7 @@ __global__ void __launch_bounds__(TC_THREADS, bn_ctas_per_sm(NM16, NO16)) bneck_
   for (uint32_t i = threadIdx.x; i < a.chunks2 * a.t_stride / 16; i += blockDim.x) st_shared_v4(sT + 16 * i, make_int4(0, 0, 0, 0));
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy zeros -> visible to the MMA
 
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  pdl_trigger();
   if (warp == TC_CONSUMER_WARPS && lane == 0) {
     s_head = 0;
     for (int s = 0; s < a.stages; s++) {
@@ -1111,25 +1137,23 @@ __global__ void __launch_bounds__(TC_THREADS, bn_ctas_per_sm(NM16, NO16)) bneck_
     bulk_load_1d(sW1, a.w1, a.w1_bytes, wfull);
     bulk_load_1d(sW2, a.w2, a.w2_bytes, wfull);
   }
-  asm volatile("griddepcontrol.wait;" ::: "memory");
+  pdl_wait();
 
-  const int tiles_per_img = a.tiles_w * a.tiles_h;
   if (warp == TC_CONSUMER_WARPS) {
     // ===================== TMA producer: one ring slot (all input channel slabs) per tile =====================
     if (lane == 0) {
       int s = 0, li = 0;
       uint32_t ph = 0;
-      TileDraw td(a.tile_ctr, a.tile_batch, a.total_tiles);
-      for (; td.tile < a.total_tiles; li++) {
-        const int tile = td.tile;
-        tq_publish(s_tile, &s_head, li, tile);
-        const int img = fdiv(tile, a.m_tpi), r = tile - img * tiles_per_img;
-        const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
+      TileDraw td(a.tile_ctr, a.tile_batch, a.tg.total);
+      for (; td.tile < a.tg.total; li++) {
+        tq_publish(s_tile, &s_head, li, td.tile);
+        const TileCoord tc = tile_coord(a.tg, td.tile);
         mbar_wait(empty + 8 * s, ph ^ 1);
         mbar_arrive_expect_tx(full + 8 * s, a.chunks1 * a.x_bytes);
         for (int ch = 0; ch < a.chunks1; ch++)
-          tma_load_4d(sX + s * a.slot + ch * a.x_stride, &a.tmX, full + 8 * s, ch * a.BK1, tw * HALO_BW - 2, th * HALO_BH - 2, img);
-        if (++s == a.stages) { s = 0; ph ^= 1; }
+          tma_load_4d(sX + s * a.slot + ch * a.x_stride, &a.tmX, full + 8 * s, ch * a.BK1, tc.tw * HALO_BW - 2, tc.th * HALO_BH - 2,
+                      tc.img);
+        ring_next(s, ph, a.stages);
         td.advance();
       }
       tq_publish(s_tile, &s_head, li, -1);  // end mark
@@ -1145,8 +1169,8 @@ __global__ void __launch_bounds__(TC_THREADS, bn_ctas_per_sm(NM16, NO16)) bneck_
   for (int li = 0;; li++) {
     const int tile = tq_get(s_tile, &s_head, li);
     if (tile < 0) break;
-    const int img = fdiv(tile, a.m_tpi), r = tile - img * tiles_per_img;
-    const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
+    const int img = fdiv(tile, a.tg.m_tpi), r = tile - img * a.tg.tpi;
+    const int th = fdiv(r, a.tg.m_tw), tw = r - th * a.tg.tiles_w;
     const int h0 = th * HALO_BH, w0 = tw * HALO_BW;
     const uint32_t xslot = sX + s * a.slot;
     mbar_wait(full + 8 * s, ph);
@@ -1174,7 +1198,7 @@ __global__ void __launch_bounds__(TC_THREADS, bn_ctas_per_sm(NM16, NO16)) bneck_
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(empty + 8 * s);
-    if (++s == a.stages) { s = 0; ph ^= 1; }
+    ring_next(s, ph, a.stages);
     // t of the previous tile is free: every warpgroup retired its stage-2 MMAs before reaching this point
     consumers_sync();
 #pragma unroll
@@ -1189,13 +1213,13 @@ __global__ void __launch_bounds__(TC_THREADS, bn_ctas_per_sm(NM16, NO16)) bneck_
 #pragma unroll
         for (int J = 0; J < NM16 * 2; J++) {
           const int c = 8 * J + 2 * t4;
-          float f0 = 0.f, f1 = 0.f;
+          float2 f = make_float2(0.f, 0.f);
           if (inside) {
             const float2 b = *reinterpret_cast<const float2*>(s_bias1 + c);
-            f0 = silu_tanh(acc1[j][4 * J + 2 * h] + b.x);
-            f1 = silu_tanh(acc1[j][4 * J + 2 * h + 1] + b.y);
+            f.x = silu_tanh(acc1[j][4 * J + 2 * h] + b.x);
+            f.y = silu_tanh(acc1[j][4 * J + 2 * h + 1] + b.y);
           }
-          const __half2 v = __floats2half2_rn(f0, f1);
+          const __half2 v = __floats2half2_rn(f.x, f.y);
           st_shared_u32(sT + (c / a.BK2) * a.t_stride + sw_off((uint32_t)row, (c % a.BK2) * 2, rb2),
                         *reinterpret_cast<const uint32_t*>(&v));
         }
@@ -1217,13 +1241,12 @@ __global__ void __launch_bounds__(TC_THREADS, bn_ctas_per_sm(NM16, NO16)) bneck_
 #pragma unroll
       for (int J = 0; J < NO16 * 2; J++) {
         const int c = 8 * J + 2 * t4;
-        const float2 b = *reinterpret_cast<const float2*>(s_bias2 + c);
-        float f0 = silu_tanh(acc2[4 * J + 2 * h] + b.x), f1 = silu_tanh(acc2[4 * J + 2 * h + 1] + b.y);
+        float2 f = bias_act(acc2 + 4 * J + 2 * h, s_bias2 + c, true);
         if (a.shortcut) {
           const float2 xv = __half22float2(*reinterpret_cast<const __half2*>(&res[h][J]));
-          f0 += xv.x; f1 += xv.y;
+          f.x += xv.x; f.y += xv.y;
         }
-        *reinterpret_cast<__half2*>(orow + c) = __floats2half2_rn(f0, f1);
+        *reinterpret_cast<__half2*>(orow + c) = __floats2half2_rn(f.x, f.y);
       }
     }
   }
@@ -1240,26 +1263,13 @@ TcBneckPlan* tc_bneck_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, st
   const bool shortcut = p2.res.base != nullptr;
   if (shortcut && (p2.res.base != p1.in.base || p2.res.coff != p1.in.coff || p2.res.pitch != p1.in.pitch || p1.Cin != p2.Cout))
     return fail("shortcut is not the block input");
-  EncodeTiledFn encode = get_encode_fn(err);
-  if (!encode) return nullptr;
-  TcBneckPlan* plan = new TcBneckPlan();
+  std::unique_ptr<TcBneckPlan> plan(new TcBneckPlan());
   BnArgs& a = plan->args;
   memset(&a, 0, sizeof(a));
-  const size_t esz = 2;
-  cuuint64_t gdim[4] = {(cuuint64_t)p1.Cin, (cuuint64_t)p1.in.W, (cuuint64_t)p1.in.H, (cuuint64_t)p1.B};
-  cuuint64_t gstr[3];
-  gstr[0] = (cuuint64_t)p1.in.pitch * esz;
-  gstr[1] = gstr[0] * p1.in.W;
-  gstr[2] = gstr[1] * p1.in.H;
-  cuuint32_t box[4] = {(cuuint32_t)a1.BK, (cuuint32_t)BN_PITCH, (cuuint32_t)(HALO_BH + 4), 1}, estr[4] = {1, 1, 1, 1};
-  const CUtensorMapSwizzle swz = a1.BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (a1.BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-  CUresult cr = encode(&a.tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, reinterpret_cast<char*>(p1.in.base) + (size_t)p1.in.coff * esz,
-                       gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) {
-    delete plan;
+  const cuuint32_t box[4] = {(cuuint32_t)a1.BK, (cuuint32_t)BN_PITCH, (cuuint32_t)(HALO_BH + 4), 1}, estr[4] = {1, 1, 1, 1};
+  if (tmap_nhwc(&a.tmX, p1.in.base, p1.in.coff, p1.Cin, p1.in.W, p1.in.H, p1.B, p1.in.pitch, box, estr, row_swizzle(a1.BK * 2)) !=
+      CUDA_SUCCESS)
     return fail("cuTensorMapEncodeTiled(bottleneck input) failed");
-  }
   a.w1 = a1.wpk; a.w2 = a2.wpk;
   a.bias1 = p1.bias; a.bias2 = p2.bias;
   a.out = reinterpret_cast<__half*>(p2.out.base);
@@ -1289,17 +1299,11 @@ TcBneckPlan* tc_bneck_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, st
     a.stages = (int)std::min<size_t>(4, (budget - fixed) / a.slot);
     if (a.stages >= occ) plan->occ = occ;
   }
-  if (!plan->occ) {
-    delete plan;
-    return fail("bottleneck tile does not fit in shared memory");
-  }
+  if (!plan->occ) return fail("bottleneck tile does not fit in shared memory");
   // At one CTA per SM both stages and their epilogues run back to back with nothing to overlap them, and without a
   // shortcut the launch saves only the round trip of t: the two unfused launches measure as fast (v8n c = 64 on H100)
   // and the forward faster, so such a pair stays unfused.
-  if (plan->occ == 1 && !shortcut) {
-    delete plan;
-    return fail("one CTA per SM and no shortcut: the unfused pair is as fast");
-  }
+  if (plan->occ == 1 && !shortcut) return fail("one CTA per SM and no shortcut: the unfused pair is as fast");
   plan->smem = (size_t)a.stages * a.slot + fixed + 1024;
   dispatch_nt16(nm16, [&](auto m) {
     dispatch_nt16(no16, [&](auto o) {
@@ -1307,21 +1311,9 @@ TcBneckPlan* tc_bneck_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, st
       if constexpr (M <= BN_MAX_C / 16 && O <= BN_MAX_C / 16) plan->kernel = bneck_tc_kernel<M, O>;
     });
   });
-  cudaFuncSetAttribute(plan->kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  // plans of different shapes share an instantiation: its limit only ever grows to the largest plan made so far, so a
-  // smaller plan created later cannot make an earlier one's launch fail
-  static std::map<void (*)(BnArgs), size_t> smem_limit;
-  size_t& lim = smem_limit[plan->kernel];
-  if (plan->smem > lim) {
-    cudaError_t ce = cudaFuncSetAttribute(plan->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan->smem);
-    if (ce != cudaSuccess) {
-      delete plan;
-      return fail("cudaFuncSetAttribute(bneck_tc_kernel) failed");
-    }
-    lim = plan->smem;
-  }
-  plan->grid = tc_num_sms() * plan->occ;
-  return plan;
+  if (smem_limit((const void*)plan->kernel, plan->smem, true) != cudaSuccess) return fail("cudaFuncSetAttribute(bneck_tc_kernel) failed");
+  plan->grid = sm_count() * plan->occ;
+  return plan.release();
 }
 
 std::string tc_bneck_plan_describe(const TcBneckPlan* plan) {
@@ -1336,13 +1328,9 @@ void tc_bneck_plan_destroy(TcBneckPlan* plan) { delete plan; }  // the weight sl
 
 int tc_bneck_launch(const TcBneckPlan* plan, int B, int* tile_ctr, cudaStream_t s) {
   BnArgs a = plan->args;
-  a.tiles_w = (a.W + HALO_BW - 1) / HALO_BW;
-  a.tiles_h = (a.H + HALO_BH - 1) / HALO_BH;
-  a.total_tiles = B * a.tiles_w * a.tiles_h;
-  a.m_tpi = fdiv_magic(a.tiles_w * a.tiles_h); a.m_tw = fdiv_magic(a.tiles_w);
+  a.tg = tile_grid(B, a.H, a.W, HALO_BH, HALO_BW, 1);
   a.tile_ctr = tile_ctr;
-  const int grid = std::min(plan->grid, a.total_tiles);
-  a.tile_batch = std::max(1, std::min(8, a.total_tiles / (4 * grid)));
+  const int grid = tc_grid(plan->grid, a.tg.total, &a.tile_batch);
   YB_CUDA_CHECK(launch_pdl(plan->kernel, dim3(grid), dim3(TC_THREADS), plan->smem, s, a));
   return 0;
 }
@@ -1377,8 +1365,7 @@ struct StemArgs {
   // produced here instead of by a separate pad kernel.  pad_h2 = the padded pixel as two fp16 (already scaled).
   int src_H, src_W;
   uint32_t pad_h2;
-  int tiles_w, tiles_h, total_tiles;
-  uint64_t m_tpi, m_tw;  // magic numbers for / tiles_per_img and / tiles_w (fdiv)
+  TileGrid tg;
 };
 
 // four input columns col .. col+3 (col even, may be -2) of one row as 4 halves; `lo_ok` = col >= 0
@@ -1457,20 +1444,19 @@ __device__ __forceinline__ void stem_pass(const StemArgs& a, uint32_t smA, uint3
   wg_wait<0>();
   wg_fence_acc<W / 2>(acc[0]);
   wg_fence_acc<W / 2>(acc[1]);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 #pragma unroll
   for (int h = 0; h < 2; h++)
 #pragma unroll
     for (int e = 0; e < 2; e++) {
-      const int row = h * 64 + warp * 16 + (lane >> 2) + 8 * e;
+      const int row = acc_row(h, e);
       const int ho = th * ST_TH + (row >> 4), wo = tw * ST_TW + (row & 15);
       if (ho >= a.Ho || wo >= a.Wo) continue;
       __half* o = a.out + ((size_t)(n * a.Ho + ho) * a.Wo + wo) * a.out_pitch + a.out_coff + c0;
 #pragma unroll
       for (int J = 0; J < W / 8; J++) {
-        const int c = 8 * J + 2 * (lane & 3);
-        *reinterpret_cast<__half2*>(o + c) = __floats2half2_rn(silu_tanh(acc[h][4 * J + 2 * e] + s_bias[c0 + c]),
-                                                               silu_tanh(acc[h][4 * J + 2 * e + 1] + s_bias[c0 + c + 1]));
+        const int c = 8 * J + 2 * (threadIdx.x & 3);
+        const float2 f = bias_act(acc[h] + 4 * J + 2 * e, s_bias + c0 + c, true);
+        *reinterpret_cast<__half2*>(o + c) = __floats2half2_rn(f.x, f.y);
       }
     }
 }
@@ -1483,7 +1469,7 @@ __global__ void __launch_bounds__(ST_THREADS, 4) stem_tc_kernel(const __grid_con
   const uint32_t base = (smem_u32(st_smem) + 1023u) & ~1023u;
   const uint32_t smA = base;              // 128 rows x 128 B
   const uint32_t smB = base + 16 * 1024;  // Cout rows x 128 B
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  pdl_trigger();
   // weights -> smem with the SWIZZLE_128B pattern; the K padding of the A rows is zeroed once
   for (int i = tid; i < a.Cout * 8; i += ST_THREADS) {
     const int n = i >> 3, pc = i & 7;
@@ -1492,17 +1478,15 @@ __global__ void __launch_bounds__(ST_THREADS, 4) stem_tc_kernel(const __grid_con
   }
   for (int i = tid; i < 128 * 8; i += ST_THREADS) st_shared_v4(smA + i * 16, make_int4(0, 0, 0, 0));
   for (int i = tid; i < a.Cout; i += ST_THREADS) s_bias[i] = a.bias[i];
-  asm volatile("griddepcontrol.wait;" ::: "memory");
+  pdl_wait();
 
-  const int tiles_per_img = a.tiles_w * a.tiles_h;
   const int tx = tid & (ST_TW - 1), ty = tid / ST_TW;  // output pixel of this thread's A row
   const size_t plane = (size_t)a.src_H * a.src_W;
   const bool ragged = a.src_W != a.W || a.src_H != a.H;  // padded source: rows may be misaligned and end early
   const uint32_t pad1 = a.pad_h2 & 0xffffu;
   auto gather = [&](int tile, uint2 (&v)[9]) {
-    const int n = fdiv(tile, a.m_tpi), r = tile - n * tiles_per_img;
-    const int th = fdiv(r, a.m_tw);
-    const int ho = th * ST_TH + ty, wo = (r - th * a.tiles_w) * ST_TW + tx;
+    const TileCoord tc = tile_coord(a.tg, tile);
+    const int n = tc.img, ho = tc.th * ST_TH + ty, wo = tc.tw * ST_TW + tx;
     const bool pix_ok = ho < a.Ho && wo < a.Wo;
     const int col = 2 * wo - 2;
 #pragma unroll
@@ -1524,12 +1508,11 @@ __global__ void __launch_bounds__(ST_THREADS, 4) stem_tc_kernel(const __grid_con
     }
   };
   uint2 v[9];
-  if (blockIdx.x < a.total_tiles) gather(blockIdx.x, v);
+  if (blockIdx.x < a.tg.total) gather(blockIdx.x, v);
   const uint32_t a_row = smA + tid * 128;
   const uint32_t sw = (uint32_t)(tid & 7);
-  for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
-    const int n = fdiv(tile, a.m_tpi), r = tile - n * tiles_per_img;
-    const int th = fdiv(r, a.m_tw), tw = r - th * a.tiles_w;
+  for (int tile = blockIdx.x; tile < a.tg.total; tile += gridDim.x) {
+    const TileCoord tc = tile_coord(a.tg, tile);
     __syncthreads();  // the previous tile's MMAs have retired in every warp before its A rows are overwritten
 #pragma unroll
     for (int pc = 0; pc < 4; pc++)
@@ -1537,13 +1520,13 @@ __global__ void __launch_bounds__(ST_THREADS, 4) stem_tc_kernel(const __grid_con
     st_shared_v4(a_row + ((4u ^ sw) << 4), make_int4((int)v[8].x, (int)v[8].y, 0, 0));
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the MMA
     __syncthreads();
-    if (tile + (int)gridDim.x < a.total_tiles) gather(tile + gridDim.x, v);  // next tile's loads fly during the MMA
+    if (tile + (int)gridDim.x < a.tg.total) gather(tile + gridDim.x, v);  // next tile's loads fly during the MMA
     for (int c0 = 0; c0 < a.Cout; c0 += 64) {
       switch (min(64, a.Cout - c0)) {
-        case 64: stem_pass<64>(a, smA, smB, s_bias, c0, n, th, tw); break;
-        case 48: stem_pass<48>(a, smA, smB, s_bias, c0, n, th, tw); break;
-        case 32: stem_pass<32>(a, smA, smB, s_bias, c0, n, th, tw); break;
-        default: stem_pass<16>(a, smA, smB, s_bias, c0, n, th, tw); break;
+        case 64: stem_pass<64>(a, smA, smB, s_bias, c0, tc.img, tc.th, tc.tw); break;
+        case 48: stem_pass<48>(a, smA, smB, s_bias, c0, tc.img, tc.th, tc.tw); break;
+        case 32: stem_pass<32>(a, smA, smB, s_bias, c0, tc.img, tc.th, tc.tw); break;
+        default: stem_pass<16>(a, smA, smB, s_bias, c0, tc.img, tc.th, tc.tw); break;
       }
     }
   }
@@ -1571,22 +1554,12 @@ int launch_stem_f16(const void* in, int in_dtype, int B, int H, int W, const __h
     const unsigned short bits = *reinterpret_cast<const unsigned short*>(&pv);
     a.pad_h2 = (uint32_t)bits | ((uint32_t)bits << 16);
   }
-  a.tiles_w = (a.Wo + ST_TW - 1) / ST_TW;
-  a.tiles_h = (a.Ho + ST_TH - 1) / ST_TH;
-  a.total_tiles = B * a.tiles_w * a.tiles_h;
-  a.m_tpi = fdiv_magic(a.tiles_w * a.tiles_h); a.m_tw = fdiv_magic(a.tiles_w);
-  static bool attrs_set = false;
+  a.tg = tile_grid(B, a.Ho, a.Wo, ST_TH, ST_TW, 1);
+  void (*kernel)(StemArgs) = in_dtype == YB_U8 ? stem_tc_kernel<YB_U8> : (in_dtype == YB_F16 ? stem_tc_kernel<YB_F16> : stem_tc_kernel<YB_F32>);
   const size_t smem = 1024 + 16 * 1024 + (size_t)a.Cout * 128;
-  if (!attrs_set) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(stem_tc_kernel<YB_U8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    YB_CUDA_CHECK(cudaFuncSetAttribute(stem_tc_kernel<YB_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    YB_CUDA_CHECK(cudaFuncSetAttribute(stem_tc_kernel<YB_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    attrs_set = true;
-  }
-  const int grid = std::min(a.total_tiles, tc_num_sms() * 4);
-  if (in_dtype == YB_U8) stem_tc_kernel<YB_U8><<<grid, ST_THREADS, smem, s>>>(a);
-  else if (in_dtype == YB_F16) stem_tc_kernel<YB_F16><<<grid, ST_THREADS, smem, s>>>(a);
-  else stem_tc_kernel<YB_F32><<<grid, ST_THREADS, smem, s>>>(a);
+  YB_CUDA_CHECK(smem_limit((const void*)kernel, smem, false));
+  const int grid = std::min(a.tg.total, sm_count() * 4);
+  kernel<<<grid, ST_THREADS, smem, s>>>(a);
   YB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

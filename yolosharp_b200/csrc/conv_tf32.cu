@@ -39,23 +39,6 @@
 
 namespace yb {
 
-typedef CUresult (*TfEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static TfEncodeFn tf_encode_fn() {
-  static TfEncodeFn fn = nullptr;
-  if (fn) return fn;
-  void* p = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess || !p) {
-    cudaGetLastError();
-    return nullptr;
-  }
-  fn = (TfEncodeFn)p;
-  return fn;
-}
-
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -248,16 +231,6 @@ int tf_pack_all(const float* P, float* WF, float* WB, const TfPackDesc* dev_desc
   return YB_OK;
 }
 
-static int tf_num_sms() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return n;
-}
-
 // One launch of tf_conv_kernel.  in: NHWC (N, Hi, Wi, Kc) fp32; wpk: [taps][Nc][Kc] fp32; out addressing given by strides.
 struct TfLaunch {
   const float* in; int N, Hi, Wi, Kc;
@@ -273,7 +246,7 @@ struct TfLaunch {
 
 // desc: when set, receives one line describing the launch (yb_debug_conv_tf32)
 static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) {
-  TfEncodeFn encode = tf_encode_fn();
+  const EncodeTiledFn encode = tmap_encode_fn();
   if (!encode) { set_error("cuTensorMapEncodeTiled entry point not found"); return YB_ERR_CUDA; }
   TfArgs a;
   memset(&a, 0, sizeof(a));
@@ -343,7 +316,7 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
   // the other's load -> MMA -> epilogue bubbles, as in conv_tc_kernel.
   const size_t per_stage = (size_t)a.a_stride + a.b_stride;
   int occ = 1;
-  if (a.n_tile <= 64 && (size_t)(100 * 1024) / per_stage >= 3 && a.total_tiles >= 2 * tf_num_sms()) occ = 2;
+  if (a.n_tile <= 64 && (size_t)(100 * 1024) / per_stage >= 3 && a.total_tiles >= 2 * sm_count()) occ = 2;
   a.stages = (int)std::min<size_t>(TF_MAX_STAGES, (size_t)((occ == 2 ? 100 : 190) * 1024) / per_stage);
   if (a.stages < 2) { set_error("tf32 conv: tile does not fit in shared memory"); return YB_ERR_SHAPE; }
   const size_t smem = (size_t)a.stages * (a.a_stride + a.b_stride) + 1024;
@@ -354,7 +327,7 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
     YB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     attr_set[a.n_tile / 16] = true;
   }
-  const int grid = std::min(a.total_tiles, occ * tf_num_sms());
+  const int grid = std::min(a.total_tiles, occ * sm_count());
   if (desc) {
     char line[256];
     snprintf(line, sizeof(line), "%stf_conv_kernel BK %d chunks %d n_tile %d x%d BW %d BH %d in_stride %d flat %d ntaps %d occ %d stages %d grid %d",
@@ -671,7 +644,7 @@ static WgPlan wg_plan(int N, int H, int W, int Cin, int Cout, int k, int stride,
   // pixel splits: one CTA per SM (189 KiB of shared memory), so the grid should fill ONE wave of SMs, or two when that fills
   // them noticeably better - never a few CTAs over (ceil(2 * SMs / pairs) capped at 64 gave grids of 300 - 320 = a third
   // wave of 4 - 24 CTAs on a third of the layers, and 64-CTA grids on the 1x1 layers with <= 128 channels)
-  const int sms = tf_num_sms();
+  const int sms = sm_count();
   const int s1 = std::max(1, sms / pairs), s2 = std::max(1, 2 * sms / pairs);
   const double u1 = (double)std::min(pairs * s1, sms) / sms, u2 = (double)std::min(pairs * s2, 2 * sms) / (2.0 * sms);
   p.splits = (pairs <= sms && u2 > u1 + 0.08) ? s2 : s1;
@@ -691,7 +664,7 @@ int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W
   if (x_pitch && (x_pitch < Cin || x_pitch % 4 || ((uintptr_t)x & 15))) { set_error("tf32 wgrad: input view must be 16-byte aligned with a pitch multiple of 4"); return YB_ERR_SHAPE; }
   const int xp = x_pitch ? x_pitch : Cin;
   if (!tf_shape_ok(Cin, Cout, k, stride, pad)) { set_error("tf32 wgrad: channels must be multiples of 8, k in {1,3}, stride in {1,2}, pad = k/2"); return YB_ERR_SHAPE; }
-  TfEncodeFn encode = tf_encode_fn();
+  const EncodeTiledFn encode = tmap_encode_fn();
   if (!encode) { set_error("cuTensorMapEncodeTiled entry point not found"); return YB_ERR_CUDA; }
   const WgPlan p = wg_plan(N, H, W, Cin, Cout, k, stride, pad);
   const size_t part_bytes = (size_t)p.splits * p.co_pad * k * k * p.ci_pad * 4;
@@ -915,7 +888,7 @@ int stem3_forward(const float* x, int xc, const float* w, int N, int H, int W, i
   if (C % 8 || C > 128 || (H & 1) || (W & 1) || xc < 3) { set_error("stem conv: C % 8 == 0, C <= 128, even input size"); return YB_ERR_SHAPE; }
   const int Ho = H / 2, Wo = W / 2;
   const long long total = (long long)N * Ho * Wo * ((C + 31) / 32);
-  const int grid = (int)std::min<long long>((total + 255) / 256, tf_num_sms() * 16);
+  const int grid = (int)std::min<long long>((total + 255) / 256, sm_count() * 16);
   stem3_forward_kernel<<<grid, 256, (size_t)27 * C * sizeof(float), s>>>(x, xc, w, z, N, H, W, Ho, Wo, C);
   YB_CUDA_CHECK(cudaGetLastError());
   return 0;

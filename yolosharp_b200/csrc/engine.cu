@@ -956,6 +956,17 @@ int32_t yb_load_tensor(yb_engine* e, const char* name, int32_t dtype, int32_t nd
   return YB_OK;
 }
 
+// true when no op other than ops[i] and ops[i + 1] reads or writes buffer `buf` (the fusion passes of yb_finalize_weights)
+static bool only_pair_uses(const yb_engine* e, size_t i, int buf) {
+  for (size_t j = 0; j < e->ops.size(); j++) {
+    if (j == i || j == i + 1) continue;
+    const OpDesc& o = e->ops[j];
+    for (const VRef* r : {&o.in, &o.out, &o.res, &o.out2, &o.out3, &o.cls, &o.coef})
+      if (r->buf == buf) return false;
+  }
+  return true;
+}
+
 int32_t yb_finalize_weights(yb_engine* e) {
   if (!e) { set_error("yb_finalize_weights: null engine"); return YB_ERR_INVALID_ARG; }
   if (e->finalized) { set_error("yb_finalize_weights: already finalized"); return YB_ERR_STATE; }
@@ -1030,14 +1041,7 @@ int32_t yb_finalize_weights(yb_engine* e) {
     if (a.type != OP_CONV || b.type != OP_CONV || !a.use_tc || !b.use_tc || a.absorbed || a.bneck) continue;
     if (a.k != 3 || a.s != 1 || b.k != 3 || b.s != 1 || a.lane != b.lane) continue;
     if (b.in.buf != a.out.buf || b.in.coff != a.out.coff || b.in.C != a.out.C) continue;
-    bool single = true;
-    for (size_t j = 0; j < e->ops.size(); j++) {
-      const OpDesc& o = e->ops[j];
-      if (j == i || j == i + 1) continue;
-      for (const VRef* r : {&o.in, &o.out, &o.res, &o.out2, &o.out3, &o.cls, &o.coef})
-        if (r->buf == a.out.buf) single = false;
-    }
-    if (!single || b.res.buf == a.out.buf) continue;
+    if (!only_pair_uses(e, i, a.out.buf) || b.res.buf == a.out.buf) continue;
     std::string err;
     b.bneck = tc_bneck_plan_create(a.plan, b.plan, &err);
     if (!b.bneck) continue;
@@ -1054,14 +1058,7 @@ int32_t yb_finalize_weights(yb_engine* e) {
     if (a.type != OP_CONV || b.type != OP_CONV || !a.use_tc || !b.use_tc || a.absorbed || a.bneck || a.fold || b.bneck) continue;
     if (a.res.buf >= 0 || a.dec.mode != EPI_STORE || b.k != 1 || b.s != 1 || b.res.buf >= 0 || a.lane != b.lane) continue;
     if (b.in.buf != a.out.buf || b.in.coff != a.out.coff || b.in.C != a.out.C) continue;
-    bool single = true;
-    for (size_t j = 0; j < e->ops.size(); j++) {
-      const OpDesc& o = e->ops[j];
-      if (j == i || j == i + 1) continue;
-      for (const VRef* r : {&o.in, &o.out, &o.res, &o.out2, &o.out3, &o.cls, &o.coef})
-        if (r->buf == a.out.buf) single = false;
-    }
-    if (!single) continue;
+    if (!only_pair_uses(e, i, a.out.buf)) continue;
     std::string err;
     b.fold = tc_fold_plan_create(a.plan, b.plan, &err);
     if (!b.fold) {

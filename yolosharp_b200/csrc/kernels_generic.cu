@@ -343,8 +343,8 @@ __global__ void __launch_bounds__(512) sppf_pool_h8_kernel(View in, View o5, Vie
   int4* cur = sp8;
   int4* tmp = sp8 + HW;
   const int n = blockIdx.y, c0 = blockIdx.x * 8;
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
+  pdl_trigger();
+  pdl_wait();
   const __half* src = reinterpret_cast<const __half*>(in.base) + (size_t)n * HW * in.pitch + in.coff + c0;
   for (int p = threadIdx.x; p < HW; p += blockDim.x) cur[p] = *reinterpret_cast<const int4*>(src + (size_t)p * in.pitch);
   __syncthreads();
