@@ -294,7 +294,10 @@ int32_t yb_dwconv3x3_backward_f32(const float* x, const float* dz, const float* 
                                   int32_t channels, float* dx, float* dw, void* stream);
 /* Replaces (training path of YOLOv11): the attention core of `Block.Attention.forward` (Modules/Block.cs:785-809):
  * out[b, i, h, :] = sum_j softmax_j(scale * q[b, i, h, :] . k[b, j, h, :]) v[b, j, h, :], and its backward.
- *   q, k, dq, dk  dev float32 (B, N, heads, key_dim);  v, out, dout, dv  dev float32 (B, N, heads, head_dim) */
+ *   q, k, dq, dk  dev float32 (B, N, heads, key_dim);  v, out, dout, dv  dev float32 (B, N, heads, head_dim)
+ * Limits (forward and backward): key_dim <= 64, head_dim <= 128, and 8 N + 32 (key_dim + 1) + 32 head_dim floats
+ * <= 200 KiB, i.e. N <= 6012 tokens at key_dim 32, head_dim 64 (YOLOv11 up to 2464 x 2464); beyond them
+ * YB_ERR_SHAPE with the limit in yb_last_error(). */
 int32_t yb_attention_forward_f32(const float* q, const float* k, const float* v, int32_t batch, int32_t tokens, int32_t heads,
                                  int32_t key_dim, int32_t head_dim, float scale, float* out, void* stream);
 int32_t yb_attention_backward_f32(const float* q, const float* k, const float* v, const float* dout, int32_t batch, int32_t tokens,

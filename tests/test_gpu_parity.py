@@ -394,6 +394,16 @@ def test_v11n_layers_and_pred(y, prec, flags, tol, ptol):
         assert float(err[:, :4].max()) < ptol[0] and float(err[:, 4:].max()) < ptol[1]
 
 
+@pytest.mark.parametrize("prec,tol", [("f32", 1e-4), ("f16", 3e-2)])
+def test_v11n_layers_704_general_attention(y, prec, tol):
+    """At 704 x 704 the C2PSA attention (model.10) runs on 22 x 22 = 484 tokens, more than the register-blocked kernel
+    takes (424), so this covers the general attention kernel of the engine."""
+    m = oracle_model("v11", "detect", "n")
+    x = synth_image(1, 704, 704)
+    e = make_engine(y, m, prec, 1, 704, 704, arch="v11")
+    check_layers(e, m, x, tol, 1, min_ops=80)
+
+
 def test_v11s_fp32_pred(y):
     """configs[3] architecture (YOLOv11s; forward only - the train step is not built yet)."""
     m = oracle_model("v11", "detect", "s")

@@ -267,7 +267,7 @@ def test_early_stopping_and_epoch_tail():
 
 @pytest.mark.gpu
 def test_train_step_v11_kernels_gpu():
-    """The same comparison with the library's kernels (csrc/train_v11.cu: depthwise conv + attention forward / backward,
+    """The same comparison with the library's kernels (csrc/train_v11.cu, csrc/attention.cu: depthwise conv + attention forward / backward,
     plus the fp32 parity kernels of the v8 step): BASELINE configs[3] architecture (n size), one full step."""
     import yolosharp_b200  # noqa: F401
     from yolosharp_b200.train_v11 import KernelOpsV11, TrainStepV11
@@ -283,7 +283,9 @@ def test_train_step_v11_tensor_cores_gpu():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("shape", [(2, 20, 20, 256), (3, 9, 7, 48), (1, 40, 40, 128)])
+@pytest.mark.parametrize("shape", [(2, 20, 20, 256), (3, 9, 7, 48), (1, 40, 40, 128),
+                                   (2, 9, 11, 30),      # C % 4 != 0: the scalar forward, dgrad and wgrad partial
+                                   (1, 5, 6, 1368)])    # C % 4 == 0 but the row kernel's weight tile (9 C floats) > 48 KiB
 def test_dwconv3x3_forward_backward_vs_autograd(shape):
     import yolosharp_b200 as y
     g = torch.Generator().manual_seed(sum(shape))
@@ -301,7 +303,11 @@ def test_dwconv3x3_forward_backward_vs_autograd(shape):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("B,N,nh,kd,hd", [(2, 400, 2, 32, 64), (3, 49, 4, 16, 32), (1, 130, 1, 32, 64)])
+# kd = 32 / hd = 64 runs the register-blocked forward up to N = 424 tokens and the register-blocked backward up to 448;
+# every other shape runs the general kernels
+@pytest.mark.parametrize("B,N,nh,kd,hd", [(2, 400, 2, 32, 64), (3, 49, 4, 16, 32), (1, 130, 1, 32, 64),
+                                          (2, 440, 2, 32, 64),   # general forward, register-blocked backward
+                                          (1, 600, 2, 32, 64)])  # general forward and backward
 def test_attention_forward_backward_vs_autograd(B, N, nh, kd, hd):
     import yolosharp_b200 as y
     from tests.torch_train_ops import TorchOps
@@ -316,3 +322,27 @@ def test_attention_forward_backward_vs_autograd(B, N, nh, kd, hd):
     dq, dk, dv = y.engine.attention_backward(q.cuda(), k.cuda(), v.cuda(), scale, do.cuda())
     for got, exp in ((dq, rq), (dk, rk), (dv, rv)):
         np.testing.assert_allclose(got.cpu().numpy(), exp.numpy(), rtol=1e-3, atol=2e-5)
+
+
+@pytest.mark.gpu
+def test_attention_shape_limits():
+    """key_dim <= 64, head_dim <= 128 and 8 N + 32 (key_dim + 1) + 32 head_dim floats <= 200 KiB (N <= 6 012 at 32 / 64),
+    for the forward and the backward alike; beyond them YB_ERR_SHAPE with the limit in the message."""
+    import yolosharp_b200 as y
+    from tests.torch_train_ops import TorchOps
+    g = torch.Generator().manual_seed(7)
+
+    def qkvo(N, kd, hd):
+        return [torch.randn(1, N, 1, d, generator=g).cuda() for d in (kd, kd, hd, hd)]
+
+    for N, kd, hd, what in ((16, 96, 64, "key_dim <= 64"), (16, 32, 160, "head_dim <= 128"), (6013, 32, 64, "limit of 6012")):
+        q, k, v, do = qkvo(N, kd, hd)
+        for call in (lambda: y.engine.attention_forward(q, k, v, kd ** -0.5),
+                     lambda: y.engine.attention_backward(q, k, v, kd ** -0.5, do)):
+            with pytest.raises(y.YbError) as ei:
+                call()
+            assert ei.value.status == -6 and what in str(ei.value), str(ei.value)
+    q, k, v, do = qkvo(6012, 32, 64)
+    out = y.engine.attention_forward(q, k, v, 32 ** -0.5)
+    ref = TorchOps._attn(q.cpu(), k.cpu(), v.cpu(), 32 ** -0.5)
+    np.testing.assert_allclose(out.cpu().numpy(), ref.numpy(), rtol=1e-4, atol=1e-5)

@@ -8,7 +8,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libyolob200.so")
-SOURCES = ["engine.cu", "kernels_generic.cu", "nms.cu", "conv_tc.cu", "loss.cu", "bn_train.cu", "comm.cu", "train_v11.cu", "ckpt.cu", "val.cu", "conv_tf32.cu", "topk.cu", "heads.cu", "train_step.cu", "metrics.cu", "segloss.cu"]
+SOURCES = ["engine.cu", "kernels_generic.cu", "nms.cu", "conv_tc.cu", "loss.cu", "bn_train.cu", "comm.cu", "train_v11.cu", "attention.cu", "ckpt.cu", "val.cu", "conv_tf32.cu", "topk.cu", "heads.cu", "train_step.cu", "metrics.cu", "segloss.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 

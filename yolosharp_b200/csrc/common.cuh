@@ -5,6 +5,7 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 #include <string>
+#include <vector>
 
 #include "yolob200.h"
 
@@ -93,6 +94,14 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(static_cast<Args&&>(args))...);
 }
+
+// storage type <-> fp32 for the kernels templated on T = float | __half
+template <typename T> __device__ __forceinline__ float to_f(T v);
+template <> __device__ __forceinline__ float to_f<float>(float v) { return v; }
+template <> __device__ __forceinline__ float to_f<__half>(__half v) { return __half2float(v); }
+template <typename T> __device__ __forceinline__ T from_f(float v);
+template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
+template <> __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
 #endif
 
 // ---- kernels_generic.cu : CUDA-core kernels, templated on storage type (float | __half) ----
@@ -122,26 +131,6 @@ int launch_decode_level(const View& box, const View& cls, const View* coef, int 
                         cudaStream_t s);
 template <typename T>
 int launch_pixel_shuffle2(const View& in, const View& out, int B, cudaStream_t s);
-// C2PSA attention core: qkv (B,N,nh*(2kd+hd)) -> out (B,N,nh*hd) and the dense v copy for the pe conv
-template <typename T>
-int launch_attention(const View& qkv, const View& out, const View& vout, int B, int nh, int kd, int hd, float scale,
-                     cudaStream_t s);
-// Tiled attention forward for kd = 32, hd = 64 (every YOLOv11 size: num_heads = c / 64, key_dim = 32), shared by the
-// inference engine (T = __half / float, q|k|v interleaved per head in the qkv conv output) and the training step (fp32,
-// separate q, k, v): element strides describe where token t of head h of image b lives.
-struct AttnIO {
-  const void *q, *k, *v;          // element type T
-  long long in_tok, in_img;       // element strides between tokens / images of q and k
-  long long v_tok, v_img;         // the same for v
-  long long q_head, k_head, v_head;  // element offset of head h: h * q_head etc. (already includes nothing else)
-  void* out;                      // type T, (B, N, nh * 64)-like with out_tok / out_img / head offset h * 64
-  long long out_tok, out_img;
-  void* vout;                     // optional dense copy of v (same addressing as out), type T
-  float *row_max, *row_sum;       // optional (B, nh, N) fp32 softmax statistics for the backward pass
-};
-template <typename T>
-int launch_attention_tiled_32x64(const AttnIO& io, int B, int N, int nh, float scale, cudaStream_t s);
-bool attention_tiled_32x64_fits(int N);
 // proto (B,h,w,32) NHWC T -> (B,32,h,w) fp32
 template <typename T>
 int launch_proto_out(const View& in, float* out, int B, cudaStream_t s);
@@ -200,5 +189,45 @@ int conv_backward_weight(const float* x, const float* dz, int N, int H, int W, i
                          float* dw, cudaStream_t s);
 int masks_launch(const float* proto, const float* dets, const int* counts, int B, int max_det, int nm,
                  int mh, int mw, int H, int W, uint8_t* masks, cudaStream_t s, int mask_cap = 0);  // mask_cap: masks per image (0 = max_det)
+// false (and the error set) when no CUDA device is present: the C entry points' first check
+bool have_device(const char* who);
+
+// ---- attention.cu : C2PSA attention core (limits: key_dim <= 64, head_dim <= 128, N <= 6 012 tokens at 32 / 64) ----
+// engine: qkv (B,N,nh*(2kd+hd)) -> out (B,N,nh*hd) and the dense v copy for the pe conv
+template <typename T>
+int launch_attention(const View& qkv, const View& out, const View& vout, int B, int nh, int kd, int hd, float scale,
+                     cudaStream_t s);
+// training, fp32: q, k (B, N, nh, kd); v, out, dout (B, N, nh, hd); row_max / row_sum optional (B, nh, N)
+int attention_forward_f32(const float* q, const float* k, const float* v, int B, int N, int nh, int kd, int hd, float scale,
+                          float* out, float* row_max, float* row_sum, cudaStream_t s);
+int attention_backward_f32(const float* q, const float* k, const float* v, const float* dout, int B, int N, int nh, int kd,
+                           int hd, float scale, float* dq, float* dk, float* dv, cudaStream_t s);
+
+// ---- entry points of the native training step (train_step.cu) in the other translation units ----
+// conv_tf32.cu : TF32 tensor-core convolutions
+int tf_conv_forward(const float* x, const float* w, const float* bias, int N, int H, int W, int Cin, int Cout, int k, int stride,
+                    int pad, float* z, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, const float* prepacked,
+                    std::string* desc = nullptr);
+int tf_conv_backward_data(const float* dz, const float* w, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
+                          float* dx, float* ws, size_t ws_bytes, cudaStream_t s, const float* prepacked,
+                          std::string* desc = nullptr);
+int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
+                            float* dw, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, std::string* desc = nullptr);
+size_t tf_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, int stride);
+struct TfPackDesc { long long off, chunk0; int cout, cin, taps, pad_; };  // off: element offset in the flat buffers; chunk0: first block
+long long tf_pack_chunks(int cout, int cin, int taps);
+int tf_pack_all(const float* P, float* WF, float* WB, const TfPackDesc* dev_descs, int nd, long long total_chunks, cudaStream_t s);
+int stem3_forward(const float* x, int xc, const float* w, int N, int H, int W, int C, float* z, cudaStream_t s);
+int stem3_backward_weight(const float* x, int xc, const float* dz, int N, int H, int W, int C, float* dw, float* ws, size_t ws_bytes,
+                          cudaStream_t s);
+// loss.cu
+int detection_loss_prepare(const float* targets_host, int n_targets, int B, int nc, int H, int W, std::vector<float>& gts, int* n_max_out);
+int detection_loss_launch_dev(const float* boxes, const float* scores, int B, int nc, int reg_max, int H, int W, const float* d_gts,
+                              int n_max, int topk, float hyp_box, float hyp_cls, float hyp_dfl, float* loss_items, float* grad_boxes,
+                              float* grad_scores, unsigned char* fg_out, int* gt_idx_out, float* tscore_out, cudaStream_t s);
+// train_v11.cu : depthwise 3x3, stride 1, pad 1, fp32 NHWC
+int dwconv3x3_forward_f32(const float* x, const float* w, int N, int H, int W, int C, float* z, cudaStream_t s);
+int dwconv3x3_backward_f32(const float* x, const float* dz, const float* w, int N, int H, int W, int C, float* dx, float* dw,
+                           cudaStream_t s);
 
 }  // namespace yb

@@ -196,7 +196,6 @@ __global__ void tf_pack_weights_kernel(const float* __restrict__ w, float* __res
   }
 }
 
-struct TfPackDesc { long long off, chunk0; int cout, cin, taps, pad_; };  // off: element offset in the flat buffers; chunk0: first block
 // Every dense conv weight of a model in ONE launch (the native training step packs once per step, after the optimizer, instead
 // of once per conv call: 158 launches of the kernel above in a YOLOv11s step).  wf / wb use the SAME element offsets as the
 // checkpoint-layout tensors inside their flat buffer, so a layer's packed operands sit at WF + off and WB + off.
@@ -339,15 +338,13 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
   return 0;
 }
 
-size_t tf_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, int stride);
-
 static bool tf_shape_ok(int Cin, int Cout, int k, int stride, int pad) {
   return Cin % 8 == 0 && Cout % 8 == 0 && (k == 1 || k == 3) && (stride == 1 || stride == 2) && pad == k / 2;
 }
 
 int tf_conv_forward(const float* x, const float* w, const float* bias, int N, int H, int W, int Cin, int Cout, int k, int stride,
                     int pad, float* z, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, const float* prepacked,
-                    std::string* desc = nullptr) {
+                    std::string* desc) {
   if (x_pitch && (x_pitch < Cin || x_pitch % 4 || ((uintptr_t)x & 15))) { set_error("tf32 conv: input view must be 16-byte aligned with a pitch multiple of 4"); return YB_ERR_SHAPE; }
   if (!tf_shape_ok(Cin, Cout, k, stride, pad)) { set_error("tf32 conv: channels must be multiples of 8, k in {1,3}, stride in {1,2}, pad = k/2"); return YB_ERR_SHAPE; }
   const size_t wn = (size_t)Cout * Cin * k * k;
@@ -371,7 +368,7 @@ int tf_conv_forward(const float* x, const float* w, const float* bias, int N, in
 
 int tf_conv_backward_data(const float* dz, const float* w, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
                           float* dx, float* ws, size_t ws_bytes, cudaStream_t s, const float* prepacked,
-                          std::string* desc = nullptr) {
+                          std::string* desc) {
   if (!tf_shape_ok(Cin, Cout, k, stride, pad) || (stride == 2 && ((H | W) & 1))) {
     set_error("tf32 dgrad: channels must be multiples of 8, k in {1,3}, stride in {1,2} (even size for stride 2), pad = k/2");
     return YB_ERR_SHAPE;
@@ -660,7 +657,7 @@ size_t tf_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, in
 }
 
 int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
-                            float* dw, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, std::string* desc = nullptr) {
+                            float* dw, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, std::string* desc) {
   if (x_pitch && (x_pitch < Cin || x_pitch % 4 || ((uintptr_t)x & 15))) { set_error("tf32 wgrad: input view must be 16-byte aligned with a pitch multiple of 4"); return YB_ERR_SHAPE; }
   const int xp = x_pitch ? x_pitch : Cin;
   if (!tf_shape_ok(Cin, Cout, k, stride, pad)) { set_error("tf32 wgrad: channels must be multiples of 8, k in {1,3}, stride in {1,2}, pad = k/2"); return YB_ERR_SHAPE; }
@@ -920,16 +917,6 @@ int stem3_backward_weight(const float* x, int xc, const float* dz, int N, int H,
   return 0;
 }
 
-static bool tf_have_dev(const char* who) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error(std::string(who) + ": no CUDA device");
-    return false;
-  }
-  return true;
-}
-
 }  // namespace yb
 
 using namespace yb;
@@ -948,7 +935,7 @@ int32_t yb_conv_forward_tc(const float* x, const float* w, const float* bias, in
                            void* stream) {
   if (!x || !w || !z || !workspace) { set_error("yb_conv_forward_tc: null argument"); return YB_ERR_INVALID_ARG; }
   if (n <= 0 || height <= 0 || width <= 0 || cin <= 0 || cout <= 0) { set_error("yb_conv_forward_tc: bad shape"); return YB_ERR_SHAPE; }
-  if (!tf_have_dev("yb_conv_forward_tc")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_conv_forward_tc")) return YB_ERR_NO_DEVICE;
   return tf_conv_forward(x, w, bias, n, height, width, cin, cout, k, stride, pad, z, (float*)workspace, (size_t)workspace_bytes,
                          (cudaStream_t)stream, 0, nullptr);
 }
@@ -958,7 +945,7 @@ int32_t yb_conv_backward_data_tc(const float* dz, const float* w, int32_t n, int
                                  void* stream) {
   if (!dz || !w || !dx || !workspace) { set_error("yb_conv_backward_data_tc: null argument"); return YB_ERR_INVALID_ARG; }
   if (n <= 0 || height <= 0 || width <= 0 || cin <= 0 || cout <= 0) { set_error("yb_conv_backward_data_tc: bad shape"); return YB_ERR_SHAPE; }
-  if (!tf_have_dev("yb_conv_backward_data_tc")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_conv_backward_data_tc")) return YB_ERR_NO_DEVICE;
   return tf_conv_backward_data(dz, w, n, height, width, cin, cout, k, stride, pad, dx, (float*)workspace, (size_t)workspace_bytes,
                                (cudaStream_t)stream, nullptr);
 }
@@ -968,7 +955,7 @@ int32_t yb_conv_backward_weight_tc(const float* x, const float* dz, int32_t n, i
                                    int64_t workspace_bytes, void* stream) {
   if (!x || !dz || !dw || !workspace) { set_error("yb_conv_backward_weight_tc: null argument"); return YB_ERR_INVALID_ARG; }
   if (n <= 0 || height <= 0 || width <= 0 || cin <= 0 || cout <= 0) { set_error("yb_conv_backward_weight_tc: bad shape"); return YB_ERR_SHAPE; }
-  if (!tf_have_dev("yb_conv_backward_weight_tc")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_conv_backward_weight_tc")) return YB_ERR_NO_DEVICE;
   return tf_conv_backward_weight(x, dz, n, height, width, cin, cout, k, stride, pad, dw, (float*)workspace, (size_t)workspace_bytes,
                                  (cudaStream_t)stream, 0);
 }
@@ -992,7 +979,7 @@ int32_t yb_debug_conv_tf32(int32_t pass, const float* x, int32_t x_pitch, const 
               "even extents for a stride-2 data gradient");
     return YB_ERR_SHAPE;
   }
-  if (!tf_have_dev("yb_debug_conv_tf32")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_debug_conv_tf32")) return YB_ERR_NO_DEVICE;
   std::string d;
   float* ws = (float*)workspace;
   const size_t wsb = (size_t)workspace_bytes;
@@ -1015,14 +1002,14 @@ int32_t yb_debug_conv_tf32(int32_t pass, const float* x, int32_t x_pitch, const 
 int32_t yb_stem_conv_forward_f32(const float* x, int32_t x_channels, const float* w, int32_t n, int32_t height, int32_t width,
                                  int32_t cout, float* z, void* stream) {
   if (!x || !w || !z || n <= 0 || height <= 0 || width <= 0 || cout <= 0) { set_error("yb_stem_conv_forward_f32: bad argument"); return YB_ERR_INVALID_ARG; }
-  if (!tf_have_dev("yb_stem_conv_forward_f32")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_stem_conv_forward_f32")) return YB_ERR_NO_DEVICE;
   return stem3_forward(x, x_channels, w, n, height, width, cout, z, (cudaStream_t)stream);
 }
 
 int32_t yb_stem_conv_backward_weight_f32(const float* x, int32_t x_channels, const float* dz, int32_t n, int32_t height, int32_t width,
                                          int32_t cout, float* dw, void* workspace, int64_t workspace_bytes, void* stream) {
   if (!x || !dz || !dw || !workspace || n <= 0 || height <= 0 || width <= 0 || cout <= 0) { set_error("yb_stem_conv_backward_weight_f32: bad argument"); return YB_ERR_INVALID_ARG; }
-  if (!tf_have_dev("yb_stem_conv_backward_weight_f32")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_stem_conv_backward_weight_f32")) return YB_ERR_NO_DEVICE;
   return stem3_backward_weight(x, x_channels, dz, n, height, width, cout, dw, (float*)workspace, (size_t)workspace_bytes, (cudaStream_t)stream);
 }
 

@@ -796,6 +796,16 @@ static int run_ops(yb_engine* e, const void* in, int in_dtype, int B, float* out
   return 0;
 }
 
+bool have_device(const char* who) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    set_error(std::string(who) + ": no CUDA device");
+    return false;
+  }
+  return true;
+}
+
 }  // namespace yb
 
 // ------------------------------------------------------------------------------------------
@@ -1162,16 +1172,6 @@ int32_t yb_detection_loss(const float* boxes, const float* scores, int32_t batch
   return detection_loss_launch(boxes, scores, batch, nc, reg_max, height, width, targets_host, n_targets, topk, hyp_box,
                                hyp_cls, hyp_dfl, loss_items, grad_boxes, grad_scores, fg, gt_idx, target_score,
                                (cudaStream_t)stream);
-}
-
-static bool have_device(const char* who) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error(std::string(who) + ": no CUDA device");
-    return false;
-  }
-  return true;
 }
 
 int32_t yb_bn_silu_train_forward(const float* z, int64_t rows, int32_t channels, int32_t pitch, const float* gamma,

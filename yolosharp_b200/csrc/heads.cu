@@ -167,16 +167,6 @@ __global__ void rnms_compact_kernel(const unsigned long long* __restrict__ keys,
 
 using namespace yb;
 
-static bool hd_have_dev(const char* who) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error(std::string(who) + ": no CUDA device");
-    return false;
-  }
-  return true;
-}
-
 extern "C" {
 
 int32_t yb_obb_decode(const float* box_logits, const float* cls_logits, const float* angle_logits, const float* anchors,
@@ -185,7 +175,7 @@ int32_t yb_obb_decode(const float* box_logits, const float* cls_logits, const fl
     set_error("yb_obb_decode: bad argument");
     return YB_ERR_INVALID_ARG;
   }
-  if (!hd_have_dev("yb_obb_decode")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_obb_decode")) return YB_ERR_NO_DEVICE;
   const long long n = (long long)batch * anchors_n;
   obb_decode_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(box_logits, cls_logits, angle_logits, anchors, strides,
                                                                                     batch, anchors_n, nc, reg_max, out);
@@ -200,7 +190,7 @@ int32_t yb_pose_decode(const float* kpts, const float* anchors, const float* str
     set_error("yb_pose_decode: bad argument (keypoint_dim must be 2 or 3 and divide the channel count)");
     return YB_ERR_INVALID_ARG;
   }
-  if (!hd_have_dev("yb_pose_decode")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_pose_decode")) return YB_ERR_NO_DEVICE;
   const long long n = (long long)batch * nk * anchors_n;
   pose_decode_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(kpts, anchors, strides, batch, anchors_n, nk,
                                                                                      keypoint_dim, out);
@@ -210,7 +200,7 @@ int32_t yb_pose_decode(const float* kpts, const float* anchors, const float* str
 
 int32_t yb_probiou(const float* obb1, int32_t n, const float* obb2, int32_t m, float eps, float* out, void* stream) {
   if (!obb1 || !obb2 || !out || n < 0 || m < 0) { set_error("yb_probiou: bad argument"); return YB_ERR_INVALID_ARG; }
-  if (!hd_have_dev("yb_probiou")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_probiou")) return YB_ERR_NO_DEVICE;
   const long long t = (long long)n * m;
   if (t == 0) return YB_OK;
   probiou_kernel<<<(unsigned)((t + 255) / 256), 256, 0, (cudaStream_t)stream>>>(obb1, n, obb2, m, eps, out);
@@ -221,7 +211,7 @@ int32_t yb_probiou(const float* obb1, int32_t n, const float* obb2, int32_t m, f
 int32_t yb_nms_rotated(const float* boxes, const float* scores, int32_t n, float threshold, int32_t* keep, int32_t* count,
                        void* stream) {
   if (!keep || !count || n < 0 || (n > 0 && (!boxes || !scores))) { set_error("yb_nms_rotated: bad argument"); return YB_ERR_INVALID_ARG; }
-  if (!hd_have_dev("yb_nms_rotated")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_nms_rotated")) return YB_ERR_NO_DEVICE;
   cudaStream_t s = (cudaStream_t)stream;
   if (n == 0) {
     YB_CUDA_CHECK(cudaMemsetAsync(count, 0, sizeof(int32_t), s));

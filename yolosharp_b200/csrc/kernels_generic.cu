@@ -10,13 +10,6 @@
 
 namespace yb {
 
-template <typename T> __device__ __forceinline__ float to_f(T v);
-template <> __device__ __forceinline__ float to_f<float>(float v) { return v; }
-template <> __device__ __forceinline__ float to_f<__half>(__half v) { return __half2float(v); }
-template <typename T> __device__ __forceinline__ T from_f(float v);
-template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
-template <> __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
-
 __device__ __forceinline__ float silu_f(float x) {
   // x * sigmoid(x), written as x / (1 + exp(-x)) like ATen's silu kernel
   return x / (1.0f + expf(-x));
@@ -656,309 +649,5 @@ int launch_pixel_shuffle2(const View& in, const View& out, int B, cudaStream_t s
 }
 template int launch_pixel_shuffle2<float>(const View&, const View&, int, cudaStream_t);
 template int launch_pixel_shuffle2<__half>(const View&, const View&, int, cudaStream_t);
-
-// ------------------------------------------------------------------------------------------
-// C2PSA attention core (Block.cs:784-791): per (image, head)
-//   attn = softmax_j(q_i . k_j * scale);  out_i = sum_j attn_ij v_j
-// qkv is the NHWC output of the qkv conv: token t = pixel, channel = head*(2kd+hd) + [q | k | v].
-// Writes out (B,N,C) with channel head*hd + d, and the dense copy of v the positional-encoding
-// depthwise conv needs (`pe(v.reshape(B,C,H,W))`).  N = 400 tokens at 640x640: one warp per query
-// row, keys streamed through shared memory in blocks of 32.
-// ------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(256) attention_kernel(View qkv, View out, View vout, int nh, int kd, int hd, float scale) {
-  extern __shared__ float at_smem[];  // per warp: scores[N]; shared: K block [32][kd+1], V block [32][hd]
-  const int N = qkv.H * qkv.W;
-  const int b = blockIdx.z, head = blockIdx.y;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nwarps = blockDim.x >> 5;
-  const int per = 2 * kd + hd;
-  const T* base = reinterpret_cast<const T*>(qkv.base) + (size_t)b * N * qkv.pitch + qkv.coff + head * per;
-  float* sc = at_smem + (size_t)warp * N;
-  float* kblk = at_smem + (size_t)nwarps * N;
-  float* vblk = kblk + 32 * (kd + 1);
-  const int i = blockIdx.x * nwarps + warp;  // query row of this warp
-  const bool active = i < N;
-  // q_i in registers (kd <= 64: up to 2 per lane)
-  float q0 = 0.f, q1 = 0.f;
-  if (active) {
-    if (lane < kd) q0 = to_f<T>(base[(size_t)i * qkv.pitch + lane]);
-    if (lane + 32 < kd) q1 = to_f<T>(base[(size_t)i * qkv.pitch + lane + 32]);
-  }
-  // pass 1: scores
-  for (int j0 = 0; j0 < N; j0 += 32) {
-    __syncthreads();
-    for (int t = threadIdx.x; t < 32 * kd; t += blockDim.x) {
-      const int jj = t / kd, d = t - jj * kd;
-      kblk[jj * (kd + 1) + d] = (j0 + jj < N) ? to_f<T>(base[(size_t)(j0 + jj) * qkv.pitch + kd + d]) : 0.f;
-    }
-    __syncthreads();
-    if (active) {
-      // lane = key j0+lane: dot(q_i, k_j) with q broadcast by shuffles
-      float acc = 0.f;
-      for (int d = 0; d < kd; d++) {
-        const float qd = __shfl_sync(0xffffffffu, d < 32 ? q0 : q1, d & 31);
-        acc = fmaf(qd, kblk[lane * (kd + 1) + d], acc);
-      }
-      if (j0 + lane < N) sc[j0 + lane] = acc * scale;
-    }
-  }
-  __syncwarp();
-  float mx = -INFINITY;
-  if (active)
-    for (int j = lane; j < N; j += 32) mx = fmaxf(mx, sc[j]);
-  for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  float sum = 0.f;
-  if (active)
-    for (int j = lane; j < N; j += 32) {
-      const float e = expf(sc[j] - mx);
-      sc[j] = e;
-      sum += e;
-    }
-  for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float inv = 1.0f / sum;
-  __syncwarp();
-  // pass 2: out_i[d] = sum_j p_j v_j[d]; lane owns d = lane, lane+32, ...
-  float o0 = 0.f, o1 = 0.f, o2 = 0.f, o3 = 0.f;
-  for (int j0 = 0; j0 < N; j0 += 32) {
-    __syncthreads();
-    for (int t = threadIdx.x; t < 32 * hd; t += blockDim.x) {
-      const int jj = t / hd, d = t - jj * hd;
-      vblk[jj * hd + d] = (j0 + jj < N) ? to_f<T>(base[(size_t)(j0 + jj) * qkv.pitch + 2 * kd + d]) : 0.f;
-    }
-    __syncthreads();
-    if (active) {
-      const int jn = min(32, N - j0);
-      for (int jj = 0; jj < jn; jj++) {
-        const float pj = sc[j0 + jj];
-        if (lane < hd) o0 = fmaf(pj, vblk[jj * hd + lane], o0);
-        if (lane + 32 < hd) o1 = fmaf(pj, vblk[jj * hd + lane + 32], o1);
-        if (lane + 64 < hd) o2 = fmaf(pj, vblk[jj * hd + lane + 64], o2);
-        if (lane + 96 < hd) o3 = fmaf(pj, vblk[jj * hd + lane + 96], o3);
-      }
-    }
-  }
-  if (!active) return;
-  T* op = reinterpret_cast<T*>(out.base) + ((size_t)b * N + i) * out.pitch + out.coff + head * hd;
-  T* vp = reinterpret_cast<T*>(vout.base) + ((size_t)b * N + i) * vout.pitch + vout.coff + head * hd;
-  const T* vsrc = base + (size_t)i * qkv.pitch + 2 * kd;
-  const float ov[4] = {o0, o1, o2, o3};
-#pragma unroll
-  for (int r = 0; r < 4; r++) {
-    const int d = lane + 32 * r;
-    if (d < hd) {
-      op[d] = from_f<T>(ov[r] * inv);
-      vp[d] = vsrc[d];
-    }
-  }
-}
-
-// Tiled variant for kd = 32, hd = 64 (all YOLOv11 sizes), used when a head's K and V fit in shared memory (N <= 416
-// tokens: every 640 x 640 model).  The row kernel above re-streams K and V through shared memory for every 8 query rows
-// (6 400 CTAs x 77 KB and 100 block-wide barriers each for YOLOv11s at batch 32).  Scalar shared-memory reads would
-// make a tiled version shared-memory bound (three LDS per two FMAs).  This one is register-blocked:
-//   * a CTA (16 warps) owns 32 query rows of one (head, image); K (row stride 36 floats) and V (stride 64) stay resident as fp32
-//   * scores: a warp owns 2 query rows, held in 64 registers; a lane owns one key per block of 32 and reads its K row
-//     with 8 conflict-free LDS.128 -> 64 FMAs per 8 loads
-//   * P.V: a lane owns channels 2*lane, 2*lane+1 for both rows; per 4 keys: 4 LDS.64 of V + 2 broadcast LDS.128 of P
-//     for 16 FMAs
-// Per-output summation order is unchanged (sequential over d, then over j).
-constexpr int ATI_T = 32, ATI_KD = 32, ATI_HD = 64, ATI_LDK = 36, ATI_THREADS = 512;  // 16 warps x 2 query rows
-__device__ __forceinline__ float4 lds128(const float* p) { return *reinterpret_cast<const float4*>(p); }
-// four consecutive elements (16 / 8 bytes, aligned) as fp32: one vector load instead of four scalar ones - the scalar
-// fill of K and V made every warp instruction touch 16 sectors for 128 useful bytes and cost 2/3 of the kernel
-template <typename T> __device__ __forceinline__ float4 ld4(const T* p);
-template <> __device__ __forceinline__ float4 ld4<float>(const float* p) { return *reinterpret_cast<const float4*>(p); }
-template <> __device__ __forceinline__ float4 ld4<__half>(const __half* p) {
-  const uint2 u = *reinterpret_cast<const uint2*>(p);
-  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
-  return make_float4(a.x, a.y, b.x, b.y);
-}
-template <typename T> __device__ __forceinline__ void cp4(T* dst, const T* src);
-template <> __device__ __forceinline__ void cp4<float>(float* dst, const float* src) { *reinterpret_cast<float4*>(dst) = *reinterpret_cast<const float4*>(src); }
-template <> __device__ __forceinline__ void cp4<__half>(__half* dst, const __half* src) { *reinterpret_cast<uint2*>(dst) = *reinterpret_cast<const uint2*>(src); }
-
-template <typename T>
-__global__ void __launch_bounds__(ATI_THREADS, 1) attention_tiled_32x64_kernel(AttnIO io, int N, int nh, float scale) {
-  extern __shared__ __align__(16) float at_smem[];
-  const int NK = (N + 31) & ~31, NP = (N + 3) & ~3;
-  float* Ks = at_smem;                          // [NK][36], rows >= N zero
-  float* Vs = Ks + (size_t)NK * ATI_LDK;        // [NP][64], rows >= N zero
-  float* Qs = Vs + (size_t)NP * ATI_HD;         // [16][32]
-  float* Ps = Qs + ATI_T * ATI_KD;              // [16][NP]
-  const int i0 = blockIdx.x * ATI_T, head = blockIdx.y, b = blockIdx.z;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const T* qb = reinterpret_cast<const T*>(io.q) + (size_t)b * io.in_img + (size_t)head * io.q_head;
-  const T* kb = reinterpret_cast<const T*>(io.k) + (size_t)b * io.in_img + (size_t)head * io.k_head;
-  const T* vb = reinterpret_cast<const T*>(io.v) + (size_t)b * io.v_img + (size_t)head * io.v_head;
-  T* vo = reinterpret_cast<T*>(io.vout);
-  // fill: 4 channels per thread and step, 8 independent vector loads in flight per thread (with one CTA of 8 warps per
-  // SM a load-convert-store loop exposes the full L2 latency on every iteration: 38 iterations x ~700 cycles was 2/3 of
-  // the kernel)
-  constexpr int U = 8;
-  for (int t0 = threadIdx.x; t0 < NK * (ATI_KD / 4); t0 += ATI_THREADS * U) {
-    float4 f[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      const int t = t0 + u * ATI_THREADS, j = t >> 3, d = (t & 7) * 4;
-      f[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (t < NK * (ATI_KD / 4) && j < N) f[u] = ld4<T>(kb + (size_t)j * io.in_tok + d);
-    }
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      const int t = t0 + u * ATI_THREADS, j = t >> 3, d = (t & 7) * 4;
-      if (t < NK * (ATI_KD / 4)) *reinterpret_cast<float4*>(Ks + (size_t)j * ATI_LDK + d) = f[u];
-    }
-  }
-  for (int t0 = threadIdx.x; t0 < NP * (ATI_HD / 4); t0 += ATI_THREADS * U) {
-    float4 f[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      const int t = t0 + u * ATI_THREADS, j = t >> 4, d = (t & 15) * 4;
-      f[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (t < NP * (ATI_HD / 4) && j < N) {
-        f[u] = ld4<T>(vb + (size_t)j * io.v_tok + d);
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      const int t = t0 + u * ATI_THREADS, j = t >> 4, d = (t & 15) * 4;
-      if (t < NP * (ATI_HD / 4)) *reinterpret_cast<float4*>(Vs + (size_t)j * ATI_HD + d) = f[u];
-    }
-  }
-  // the dense copy of v that the positional-encoding conv reads: this CTA's 32 rows, one vector per thread.  (Inside the
-  // fill loop above these stores would sit between the batched loads and each wait for its own load.)
-  if (vo) {
-    const int r = threadIdx.x >> 4, d = (threadIdx.x & 15) * 4, j = i0 + r;
-    if (j < N) cp4<T>(vo + (size_t)b * io.out_img + (size_t)j * io.out_tok + head * ATI_HD + d, vb + (size_t)j * io.v_tok + d);
-  }
-  for (int t = threadIdx.x; t < ATI_T * ATI_KD; t += ATI_THREADS) {
-    const int r = t >> 5, d = t & 31;
-    Qs[t] = (i0 + r < N) ? to_f<T>(qb[(size_t)(i0 + r) * io.in_tok + d]) : 0.f;
-  }
-  __syncthreads();
-  const int r0 = warp * 2, r1 = r0 + 1;
-  float* p0 = Ps + (size_t)r0 * NP;
-  float* p1 = Ps + (size_t)r1 * NP;
-  float q0[ATI_KD], q1[ATI_KD];
-#pragma unroll
-  for (int d = 0; d < ATI_KD; d += 4) {
-    const float4 a = lds128(Qs + r0 * ATI_KD + d), c = lds128(Qs + r1 * ATI_KD + d);
-    q0[d] = a.x; q0[d + 1] = a.y; q0[d + 2] = a.z; q0[d + 3] = a.w;
-    q1[d] = c.x; q1[d + 1] = c.y; q1[d + 2] = c.z; q1[d + 3] = c.w;
-  }
-  float m0 = -INFINITY, m1 = -INFINITY;
-  for (int j = lane; j < NK; j += 32) {
-    const float* kr = Ks + (size_t)j * ATI_LDK;
-    float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-    for (int d = 0; d < ATI_KD; d += 4) {
-      const float4 kv = lds128(kr + d);
-      s0 = fmaf(q0[d], kv.x, s0); s1 = fmaf(q1[d], kv.x, s1);
-      s0 = fmaf(q0[d + 1], kv.y, s0); s1 = fmaf(q1[d + 1], kv.y, s1);
-      s0 = fmaf(q0[d + 2], kv.z, s0); s1 = fmaf(q1[d + 2], kv.z, s1);
-      s0 = fmaf(q0[d + 3], kv.w, s0); s1 = fmaf(q1[d + 3], kv.w, s1);
-    }
-    if (j < N) {
-      s0 *= scale; s1 *= scale;
-      p0[j] = s0; p1[j] = s1;
-      m0 = fmaxf(m0, s0); m1 = fmaxf(m1, s1);
-    } else if (j < NP) {
-      p0[j] = -INFINITY; p1[j] = -INFINITY;  // exp -> 0: padded keys contribute nothing
-    }
-  }
-  for (int o = 16; o; o >>= 1) { m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o)); }
-  float l0 = 0.f, l1 = 0.f;
-  for (int j = lane; j < NP; j += 32) {
-    const float e0 = expf(p0[j] - m0), e1 = expf(p1[j] - m1);
-    p0[j] = e0; p1[j] = e1;
-    l0 += e0; l1 += e1;
-  }
-  for (int o = 16; o; o >>= 1) { l0 += __shfl_xor_sync(0xffffffffu, l0, o); l1 += __shfl_xor_sync(0xffffffffu, l1, o); }
-  __syncwarp();
-  float a00 = 0.f, a01 = 0.f, a10 = 0.f, a11 = 0.f;
-  const float* vcol = Vs + 2 * lane;
-  for (int j = 0; j < NP; j += 4) {
-    const float4 pa = lds128(p0 + j), pb = lds128(p1 + j);
-    const float2 v0 = *reinterpret_cast<const float2*>(vcol + (size_t)j * ATI_HD);
-    const float2 v1 = *reinterpret_cast<const float2*>(vcol + (size_t)(j + 1) * ATI_HD);
-    const float2 v2 = *reinterpret_cast<const float2*>(vcol + (size_t)(j + 2) * ATI_HD);
-    const float2 v3 = *reinterpret_cast<const float2*>(vcol + (size_t)(j + 3) * ATI_HD);
-    a00 = fmaf(pa.x, v0.x, a00); a01 = fmaf(pa.x, v0.y, a01); a10 = fmaf(pb.x, v0.x, a10); a11 = fmaf(pb.x, v0.y, a11);
-    a00 = fmaf(pa.y, v1.x, a00); a01 = fmaf(pa.y, v1.y, a01); a10 = fmaf(pb.y, v1.x, a10); a11 = fmaf(pb.y, v1.y, a11);
-    a00 = fmaf(pa.z, v2.x, a00); a01 = fmaf(pa.z, v2.y, a01); a10 = fmaf(pb.z, v2.x, a10); a11 = fmaf(pb.z, v2.y, a11);
-    a00 = fmaf(pa.w, v3.x, a00); a01 = fmaf(pa.w, v3.y, a01); a10 = fmaf(pb.w, v3.x, a10); a11 = fmaf(pb.w, v3.y, a11);
-  }
-  const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
-  T* ob = reinterpret_cast<T*>(io.out) + (size_t)b * io.out_img + head * ATI_HD + 2 * lane;
-  if (i0 + r0 < N) { T* o = ob + (size_t)(i0 + r0) * io.out_tok; o[0] = from_f<T>(a00 * inv0); o[1] = from_f<T>(a01 * inv0); }
-  if (i0 + r1 < N) { T* o = ob + (size_t)(i0 + r1) * io.out_tok; o[0] = from_f<T>(a10 * inv1); o[1] = from_f<T>(a11 * inv1); }
-  if (lane == 0 && io.row_max) {
-    if (i0 + r0 < N) { io.row_max[((size_t)b * nh + head) * N + i0 + r0] = m0; io.row_sum[((size_t)b * nh + head) * N + i0 + r0] = l0; }
-    if (i0 + r1 < N) { io.row_max[((size_t)b * nh + head) * N + i0 + r1] = m1; io.row_sum[((size_t)b * nh + head) * N + i0 + r1] = l1; }
-  }
-}
-
-static size_t ati_smem_bytes(int N) {
-  const size_t NK = (N + 31) & ~31, NP = (N + 3) & ~3;
-  return (NK * ATI_LDK + NP * ATI_HD + (size_t)ATI_T * ATI_KD + (size_t)ATI_T * NP) * sizeof(float);
-}
-bool attention_tiled_32x64_fits(int N) { return ati_smem_bytes(N) <= 227 * 1024; }
-
-template <typename T>
-int launch_attention_tiled_32x64(const AttnIO& io, int B, int N, int nh, float scale, cudaStream_t s) {
-  static bool attr = false;
-  if (!attr) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(attention_tiled_32x64_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr = true;
-  }
-  attention_tiled_32x64_kernel<T><<<dim3((N + ATI_T - 1) / ATI_T, nh, B), ATI_THREADS, ati_smem_bytes(N), s>>>(io, N, nh, scale);
-  YB_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
-template int launch_attention_tiled_32x64<float>(const AttnIO&, int, int, int, float, cudaStream_t);
-template int launch_attention_tiled_32x64<__half>(const AttnIO&, int, int, int, float, cudaStream_t);
-
-template <typename T>
-int launch_attention(const View& qkv, const View& out, const View& vout, int B, int nh, int kd, int hd, float scale,
-                     cudaStream_t s) {
-  const int N = qkv.H * qkv.W;
-  if (kd > 64 || hd > 128) {
-    set_error("attention: key_dim <= 64 and head_dim <= 128 supported");
-    return YB_ERR_SHAPE;
-  }
-  if (kd == ATI_KD && hd == ATI_HD && attention_tiled_32x64_fits(N) && qkv.pitch % 4 == 0 && qkv.coff % 4 == 0 &&
-      out.pitch % 4 == 0 && out.coff % 4 == 0 && vout.coff % 4 == 0) {
-    const int per = 2 * kd + hd;
-    AttnIO io;
-    const T* base = reinterpret_cast<const T*>(qkv.base) + qkv.coff;
-    io.q = base; io.k = base + kd; io.v = base + 2 * kd;
-    io.in_tok = io.v_tok = qkv.pitch; io.in_img = io.v_img = (long long)N * qkv.pitch;
-    io.q_head = io.k_head = io.v_head = per;
-    io.out = reinterpret_cast<T*>(out.base) + out.coff; io.out_tok = out.pitch; io.out_img = (long long)N * out.pitch;
-    io.vout = reinterpret_cast<T*>(vout.base) + vout.coff;
-    io.row_max = io.row_sum = nullptr;
-    if (vout.pitch != out.pitch) { set_error("attention: out and v copy must share their pitch"); return YB_ERR_SHAPE; }
-    return launch_attention_tiled_32x64<T>(io, B, N, nh, scale, s);
-  }
-  const int nwarps = 8;
-  const size_t smem = ((size_t)nwarps * N + 32 * (kd + 1) + 32 * hd) * sizeof(float);
-  if (smem > 200 * 1024) {
-    set_error("attention: too many tokens for the shared-memory kernel");
-    return YB_ERR_SHAPE;
-  }
-  static bool attr_set[2] = {false, false};
-  const int ti = sizeof(T) == 4 ? 0 : 1;
-  if (!attr_set[ti]) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set[ti] = true;
-  }
-  dim3 grid((N + nwarps - 1) / nwarps, nh, B);
-  attention_kernel<T><<<grid, nwarps * 32, smem, s>>>(qkv, out, vout, nh, kd, hd, scale);
-  YB_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
-template int launch_attention<float>(const View&, const View&, const View&, int, int, int, int, float, cudaStream_t);
-template int launch_attention<__half>(const View&, const View&, const View&, int, int, int, int, float, cudaStream_t);
 
 }  // namespace yb

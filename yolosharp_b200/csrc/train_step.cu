@@ -9,7 +9,8 @@
 //   dense convolutions   TF32 tensor-core forward / dgrad / wgrad (csrc/conv_tf32.cu); the 3-channel stem runs with its
 //                        input zero-padded to 8 channels
 //   BatchNorm + SiLU     csrc/bn_train.cu (batch statistics, running-stat update, backward)
-//   depthwise 3x3, attention   csrc/train_v11.cu
+//   depthwise 3x3        csrc/train_v11.cu
+//   attention core       csrc/attention.cu
 //   everything between   small kernels below: channel-slice copies (concat / chunk), adds, nearest-2x upsample and its
 //                        backward, MaxPool2d(5,1,2) with saved argmax and a gather-form (deterministic) backward, the
 //                        NHWC <-> (B, C, A) head transposes, per-channel sums for the conv biases
@@ -27,34 +28,6 @@
 #include "common.cuh"
 
 namespace yb {
-
-// entry points of the other translation units this step is made of
-int tf_conv_forward(const float* x, const float* w, const float* bias, int N, int H, int W, int Cin, int Cout, int k, int stride,
-                    int pad, float* z, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, const float* prepacked,
-                    std::string* desc = nullptr);
-int tf_conv_backward_data(const float* dz, const float* w, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
-                          float* dx, float* ws, size_t ws_bytes, cudaStream_t s, const float* prepacked,
-                          std::string* desc = nullptr);
-struct TfPackDesc { long long off, chunk0; int cout, cin, taps, pad_; };
-long long tf_pack_chunks(int cout, int cin, int taps);
-int tf_pack_all(const float* P, float* WF, float* WB, const TfPackDesc* dev_descs, int nd, long long total_chunks, cudaStream_t s);
-int detection_loss_prepare(const float* targets_host, int n_targets, int B, int nc, int H, int W, std::vector<float>& gts, int* n_max_out);
-int detection_loss_launch_dev(const float* boxes, const float* scores, int B, int nc, int reg_max, int H, int W, const float* d_gts,
-                              int n_max, int topk, float hyp_box, float hyp_cls, float hyp_dfl, float* loss_items, float* grad_boxes,
-                              float* grad_scores, unsigned char* fg_out, int* gt_idx_out, float* tscore_out, cudaStream_t s);
-int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
-                            float* dw, float* ws, size_t ws_bytes, cudaStream_t s, int x_pitch, std::string* desc = nullptr);
-size_t tf_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, int stride);
-int stem3_forward(const float* x, int xc, const float* w, int N, int H, int W, int C, float* z, cudaStream_t s);
-int stem3_backward_weight(const float* x, int xc, const float* dz, int N, int H, int W, int C, float* dw, float* ws, size_t ws_bytes,
-                          cudaStream_t s);
-int dwconv3x3_forward_f32(const float* x, const float* w, int N, int H, int W, int C, float* z, cudaStream_t s);
-int dwconv3x3_backward_f32(const float* x, const float* dz, const float* w, int N, int H, int W, int C, float* dx, float* dw,
-                           cudaStream_t s);
-int attention_forward_f32(const float* q, const float* k, const float* v, int B, int N, int nh, int kd, int hd, float scale,
-                          float* out, float* row_max, float* row_sum, cudaStream_t s);
-int attention_backward_f32(const float* q, const float* k, const float* v, const float* dout, int B, int N, int nh, int kd,
-                           int hd, float scale, float* dq, float* dk, float* dv, cudaStream_t s);
 
 namespace ts {
 

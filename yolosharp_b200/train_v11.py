@@ -2,7 +2,8 @@
 `train.py`: the wiring, the forward/backward of C3k2 / C3k / C2PSA / PSABlock / Attention and the v11 Detect head,
 pinned against autograd through the oracle on the CPU (PyTorch stand-in of the kernel interface) and on the GPU with
 the library's kernels (tests/test_train_step.py): csrc/train_v11.cu adds the depthwise 3x3 convolution (forward,
-dgrad, wgrad) and the attention core softmax(q^T k) v with its backward to the fp32 parity kernels of the v8 step.
+dgrad, wgrad) and csrc/attention.cu the attention core softmax(q^T k) v with its backward to the fp32 parity kernels
+of the v8 step.
 
 Reference: Models/Yolo.cs:200-258 (Yolov11 wiring, outputIndexs {4,6,10,13,16,19,22}), Modules/Block.cs:404-441 (C3),
 :611-661 (C3k, C3k2), :664-810 (C2PSA, PSABlock, Attention), Modules/Convs.cs:108-114 (DWConv), Modules/Head.cs:35-53
@@ -22,7 +23,7 @@ V11_SIZES = {  # Models/Yolo.cs:213-217 (depth, width, max_channels, c3k)
 
 
 class KernelOpsV11(KernelOps):
-    """+ the depthwise 3x3 and attention kernels of csrc/train_v11.cu.  Every grouped conv of Yolov11 is depthwise
+    """+ the depthwise 3x3 (csrc/train_v11.cu) and attention (csrc/attention.cu) kernels.  Every grouped conv of Yolov11 is depthwise
     3x3 stride 1 (DWConv(c, c, 3) in the head, Attention.pe); anything else is refused, not emulated."""
 
     @staticmethod
