@@ -159,6 +159,53 @@ def _train_worker(rank, world, port, q):
         dist.destroy_process_group()
 
 
+def _two_devices_worker(q):
+    try:
+        import yolosharp_b200 as y
+        from yolosharp_b200.engine import nms
+        from yolosharp_b200.train_native import NativeTrainer
+        from tests.test_train_step import _targets
+        from tests.util import oracle_model, synth_image
+        det_sd = oracle_model("v8", "detect", "n").state_dict()
+        train_sd = {k: v.detach().clone() for k, v in oracle_model("v11", "detect", "n").state_dict().items()}
+        x, xt, t = synth_image(2, 640, 640, seed=3), synth_image(2, 128, 128, seed=4), _targets(2)
+        res = []
+        for d in (0, 1):
+            with torch.cuda.device(d):
+                e = y.Engine("v8", "n", "detect", 80, "f16", d, 2, 640, 640)
+                e.load_state_dict(det_sd)
+                e.finalize()
+                dets, counts, _ = nms(e.forward(x.cuda(d)))
+                tr = NativeTrainer(train_sd, "v11", "n", 80, device=torch.device("cuda", d), max_batch=2, height=128, width=128,
+                                   lr=1e-3)
+                items = tr.step(xt.cuda(d), t)
+                torch.cuda.synchronize()
+                res.append({"dets": dets.cpu(), "counts": counts.cpu(), "loss items": items.clone(), "grad": tr.grad.cpu()})
+                tr.close()
+                e.close()
+        # the loss items are summed over blocks with float atomics, so two runs on one device may differ in the last bit;
+        # the gradient does not depend on them and must match exactly
+        a, b = res
+        q.put([k for k in a if not (torch.allclose(a[k], b[k], rtol=1e-6, atol=0) if k == "loss items" else torch.equal(a[k], b[k]))])
+    except Exception as ex:  # a refused launch surfaces as YbError from the call that made it
+        q.put(repr(ex))
+
+
+def test_two_devices_in_one_process():
+    """An f16 engine (forward + NMS) and a v11n native training step on device 0, then the same on device 1, in one fresh
+    process: every kernel that needs more than 48 KiB of shared memory must get its limit on the second device too (the
+    limit is a per-device function attribute), and device 1 must reproduce device 0 bit for bit."""
+    _need(2)
+    ctx = mp.get_context("spawn")
+    q = ctx.Queue()
+    p = ctx.Process(target=_two_devices_worker, args=(q,))
+    p.start()
+    res = q.get(timeout=600)
+    p.join(120)
+    assert res == [], res
+    assert p.exitcode == 0
+
+
 def test_native_train_step_allreduce_world2():
     """The native step on 2 GPUs (BASELINE configs[3] mechanics): after yb_train_backward + the NCCL all-reduce of the flat
     gradient buffer every rank holds the SUM of the two shards' gradients (each equal to a single-GPU step on that shard:

@@ -307,18 +307,10 @@ template <typename T>
 static int attention_launch(const AttnIO& io, int B, int N, int nh, int kd, int hd, float scale, cudaStream_t s) {
   if (int rc = attention_check(B, N, nh, kd, hd)) return rc;
   if (kd == ATI_KD && hd == ATI_HD && ati_smem_bytes(N) <= 227 * 1024 && ati_vec4_ok<T>(io)) {
-    static bool attr = false;
-    if (!attr) {
-      YB_CUDA_CHECK(cudaFuncSetAttribute(attention_tiled_32x64_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr = true;
-    }
+    YB_CUDA_CHECK(smem_limit((const void*)attention_tiled_32x64_kernel<T>, ati_smem_bytes(N), false));
     attention_tiled_32x64_kernel<T><<<dim3((N + ATI_T - 1) / ATI_T, nh, B), ATI_THREADS, ati_smem_bytes(N), s>>>(io, N, nh, scale);
   } else {
-    static bool attr = false;
-    if (!attr) {
-      YB_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, AG_SMEM_MAX));
-      attr = true;
-    }
+    YB_CUDA_CHECK(smem_limit((const void*)attention_kernel<T>, ag_smem_bytes(N, kd, hd), false));
     attention_kernel<T><<<dim3((N + AG_WARPS - 1) / AG_WARPS, nh, B), AG_WARPS * 32, ag_smem_bytes(N, kd, hd), s>>>(io, N, nh, kd, hd, scale);
   }
   YB_CUDA_CHECK(cudaGetLastError());
@@ -698,23 +690,29 @@ int attention_backward_f32(const float* q, const float* k, const float* v, const
   YB_CUDA_CHECK(cudaMallocAsync((void**)&stats, (3 * n + (size_t)B * N * nh * hd) * sizeof(float), s));
   float* tmp_out = stats + 3 * n;  // the forward output is recomputed only for its row statistics
   int rc = attention_forward_f32(q, k, v, B, N, nh, kd, hd, scale, tmp_out, stats, stats + n, s);
+  cudaError_t ce = cudaSuccess;
   if (!rc && kd == 32 && hd == 64 && ab_fits(N)) {
-    cudaFuncSetAttribute(attn_bwd_q_32x64, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(attn_bwd_kv_32x64, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    const dim3 grid((N + AB_T - 1) / AB_T, nh, B);
-    attn_bwd_q_32x64<<<grid, AB_THREADS, ab_smem_bytes(N, 0), s>>>(q, k, v, dout, tmp_out, stats, stats + n, stats + 2 * n, dq, N, nh, scale);
-    attn_bwd_kv_32x64<<<grid, AB_THREADS, ab_smem_bytes(N, 1), s>>>(q, k, v, dout, stats, stats + n, stats + 2 * n, dk, dv, N, nh, scale);
-    if (cudaGetLastError() != cudaSuccess) { set_error("attention backward launch failed"); rc = YB_ERR_CUDA; }
+    ce = smem_limit((const void*)attn_bwd_q_32x64, ab_smem_bytes(N, 0), false);
+    if (ce == cudaSuccess) ce = smem_limit((const void*)attn_bwd_kv_32x64, ab_smem_bytes(N, 1), false);
+    if (ce == cudaSuccess) {
+      const dim3 grid((N + AB_T - 1) / AB_T, nh, B);
+      attn_bwd_q_32x64<<<grid, AB_THREADS, ab_smem_bytes(N, 0), s>>>(q, k, v, dout, tmp_out, stats, stats + n, stats + 2 * n, dq, N, nh, scale);
+      attn_bwd_kv_32x64<<<grid, AB_THREADS, ab_smem_bytes(N, 1), s>>>(q, k, v, dout, stats, stats + n, stats + 2 * n, dk, dv, N, nh, scale);
+      ce = cudaGetLastError();
+    }
   } else if (!rc) {  // shared memory: N + kd + hd (q pass) and 2 N + kd + hd (kv pass) floats, within attention_check's limit
     const size_t smem_q = ((size_t)N + kd + hd) * sizeof(float), smem_kv = ((size_t)2 * N + kd + hd) * sizeof(float);
-    cudaFuncSetAttribute(attn_backward_q_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AG_SMEM_MAX);
-    cudaFuncSetAttribute(attn_backward_kv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AG_SMEM_MAX);
-    attn_backward_q_kernel<<<dim3(N, nh, B), AT_THREADS, smem_q, s>>>(q, k, v, dout, stats, stats + n, stats + 2 * n, dq, N, nh, kd,
-                                                                       hd, scale);
-    attn_backward_kv_kernel<<<dim3(N, nh, B), AT_THREADS, smem_kv, s>>>(q, k, v, dout, stats, stats + n, stats + 2 * n, dk, dv, N, nh,
-                                                                         kd, hd, scale);
-    if (cudaGetLastError() != cudaSuccess) { set_error("attention backward launch failed"); rc = YB_ERR_CUDA; }
+    ce = smem_limit((const void*)attn_backward_q_kernel, smem_q, false);
+    if (ce == cudaSuccess) ce = smem_limit((const void*)attn_backward_kv_kernel, smem_kv, false);
+    if (ce == cudaSuccess) {
+      attn_backward_q_kernel<<<dim3(N, nh, B), AT_THREADS, smem_q, s>>>(q, k, v, dout, stats, stats + n, stats + 2 * n, dq, N, nh, kd,
+                                                                         hd, scale);
+      attn_backward_kv_kernel<<<dim3(N, nh, B), AT_THREADS, smem_kv, s>>>(q, k, v, dout, stats, stats + n, stats + 2 * n, dk, dv, N,
+                                                                           nh, kd, hd, scale);
+      ce = cudaGetLastError();
+    }
   }
+  if (ce != cudaSuccess) { set_error("attention backward launch failed"); rc = YB_ERR_CUDA; }
   cudaFreeAsync(stats, s);
   return rc;
 }

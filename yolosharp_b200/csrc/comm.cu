@@ -104,11 +104,7 @@ int32_t yb_comm_create(int32_t rank, int32_t world, int32_t device, int64_t byte
   if (slots < 1 || slots > COMM_MAX_SLOTS) { set_error("yb_comm_create: slots outside [1,8]"); return YB_ERR_INVALID_ARG; }
   if (bytes_per_rank <= 0 || bytes_per_rank % 16 || bytes_per_rank > (1ll << 30)) { set_error("yb_comm_create: bytes_per_rank must be a positive multiple of 16 (<= 1 GiB)"); return YB_ERR_INVALID_ARG; }
   int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error("yb_comm_create: no CUDA device");
-    return YB_ERR_NO_DEVICE;
-  }
+  if (!have_device("yb_comm_create", &ndev)) return YB_ERR_NO_DEVICE;
   if (device < 0 || device >= ndev) { set_error("yb_comm_create: bad device ordinal"); return YB_ERR_INVALID_ARG; }
   YB_CUDA_CHECK(cudaSetDevice(device));
   std::unique_ptr<yb_comm> c(new yb_comm());

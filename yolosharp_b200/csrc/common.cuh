@@ -136,13 +136,23 @@ template <typename T>
 int launch_proto_out(const View& in, float* out, int B, cudaStream_t s);
 
 // ---- conv_tc.cu : wgmma implicit-GEMM conv (fp16 storage, fp32 accumulate) ----
-// Device queries shared by the tensor-core convolutions of conv_tc.cu and conv_tf32.cu, cached after the first call:
-// the driver's cuTensorMapEncodeTiled (nullptr when the entry point is missing) and the SM count of the current device.
+// Device queries, cached after the first call: the driver's cuTensorMapEncodeTiled (nullptr when the entry point is
+// missing) and the SM count of the current device (one value per device).
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn tmap_encode_fn();
 int sm_count();
+// 4-D tensor map {C, W, H, N} of an NHWC buffer of `type` (FLOAT16 or FLOAT32) elements whose pixels are `pitch` channels
+// apart, starting at channel coff
+CUresult tmap_nhwc(CUtensorMap* map, CUtensorMapDataType type, void* base, int coff, int C, int W, int H, int N, int pitch,
+                   const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapSwizzle swz);
+// Dynamic shared-memory limit of `kernel` on the current device for a launch of `smem` bytes, and for the persistent
+// ring kernels (max_carveout) the largest carveout.  Every kernel whose launch needs more than 48 KiB sets its limit
+// here.  Launches of different sizes share a kernel: its limit (per device) only ever grows to the largest launch so far,
+// so a smaller launch set up later cannot make an earlier one fail.  cudaFuncSetAttribute acts on the current device only,
+// so the limit is kept per (device, kernel).
+cudaError_t smem_limit(const void* kernel, size_t smem, bool max_carveout);
 struct TcConvPlan;  // opaque: tensor maps + tiling for one conv layer
 TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err);
 void tc_conv_plan_destroy(TcConvPlan* plan);
@@ -189,8 +199,8 @@ int conv_backward_weight(const float* x, const float* dz, int N, int H, int W, i
                          float* dw, cudaStream_t s);
 int masks_launch(const float* proto, const float* dets, const int* counts, int B, int max_det, int nm,
                  int mh, int mw, int H, int W, uint8_t* masks, cudaStream_t s, int mask_cap = 0);  // mask_cap: masks per image (0 = max_det)
-// false (and the error set) when no CUDA device is present: the C entry points' first check
-bool have_device(const char* who);
+// false (and the error set) when no CUDA device is present: the C entry points' first check.  ndev: the device count.
+bool have_device(const char* who, int* ndev = nullptr);
 
 // ---- attention.cu : C2PSA attention core (limits: key_dim <= 64, head_dim <= 128, N <= 6 012 tokens at 32 / 64) ----
 // engine: qkv (B,N,nh*(2kd+hd)) -> out (B,N,nh*hd) and the dense v copy for the pe conv

@@ -35,26 +35,6 @@
 
 namespace yb {
 
-// exact x / d for x*d < 2^40 as (x * ceil(2^40/d)) >> 40 (runtime integer division costs ~100+ cycles)
-__device__ __forceinline__ int fdiv(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
-// the host side of fdiv: ceil(2^40 / d)
-static uint64_t fdiv_magic(int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); }
-
-// The tiles of one launch: `imgs` images of tiles_h x tiles_w output rectangles, each split into n_tiles N tiles.  Tile
-// index = ((img * tiles_h + th) * tiles_w + tw) * n_tiles + nt; the magic numbers divide by n_tiles, tpi and tiles_w.
-struct TileGrid {
-  int tiles_w, tpi, n_tiles, total;  // tpi = tiles per image
-  uint64_t m_ntiles, m_tpi, m_tw;
-};
-static TileGrid tile_grid(int imgs, int H, int W, int BH, int BW, int n_tiles) {
-  TileGrid g;
-  g.tiles_w = (W + BW - 1) / BW;
-  g.tpi = g.tiles_w * ((H + BH - 1) / BH);
-  g.n_tiles = n_tiles;
-  g.total = imgs * g.tpi * n_tiles;
-  g.m_ntiles = fdiv_magic(n_tiles); g.m_tpi = fdiv_magic(g.tpi); g.m_tw = fdiv_magic(g.tiles_w);
-  return g;
-}
 // Grid of a persistent launch of `total` tiles on at most `max_grid` CTAs, and the tiles per draw from the launch's
 // counter: one atomic per ~quarter of a CTA's share (every atomic of the grid hits the same L2 address, so per-tile
 // draws would serialise the 6400-tile layers)
@@ -62,13 +42,6 @@ static int tc_grid(int max_grid, int total, int* tile_batch) {
   const int grid = std::min(max_grid, total);
   *tile_batch = std::max(1, std::min(8, total / (4 * grid)));
   return grid;
-}
-struct TileCoord { int img, th, tw, nt; };
-__device__ __forceinline__ TileCoord tile_coord(const TileGrid& g, int tile) {
-  const int mt = fdiv(tile, g.m_ntiles);
-  const int img = fdiv(mt, g.m_tpi), r = mt - img * g.tpi;
-  const int th = fdiv(r, g.m_tw);
-  return {img, th, r - th * g.tiles_w, tile - mt * g.n_tiles};
 }
 
 enum TcMode { TC_TAP = 0, TC_HALO = 1, TC_S2P = 2 };
@@ -151,29 +124,9 @@ __device__ __forceinline__ float2 bias_act(const float* acc, const float* bias, 
   return f;
 }
 
-// Row of accumulator half h of this thread in m64 block `blk` of a tile (wgmma D fragment, tc_ptx.cuh)
-__device__ __forceinline__ int acc_row(int blk, int h) {
-  return blk * 64 + ((threadIdx.x >> 5) & 3) * 16 + ((threadIdx.x & 31) >> 2) + 8 * h;
-}
-
 // Descriptor start shift (16-byte units) of 3x3 tap t inside a staged tile of `pitch`-pixel rows, row16 units per pixel
 __device__ __forceinline__ uint32_t tap_shift(int t, int pitch, uint32_t row16) {
   return (uint32_t)((t / 3) * pitch + t % 3) * row16;
-}
-
-// Next slot of an n-slot mbarrier ring; the wait parity flips on every wrap
-__device__ __forceinline__ void ring_next(int& s, uint32_t& ph, int n) {
-  if (++s == n) { s = 0; ph ^= 1; }
-}
-
-// Operand rows of 128 / 64 / 32 bytes: the tensor-map swizzle, the wgmma layout type it produces, and (device) the
-// 16-byte piece index XOR of row r under it
-static CUtensorMapSwizzle row_swizzle(int row_bytes) {
-  return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-}
-static uint32_t row_layout(int row_bytes) { return row_bytes == 128 ? 1 : (row_bytes == 64 ? 2 : 3); }
-__device__ __forceinline__ uint32_t row_swizzle_xor(uint32_t r, uint32_t row_bytes) {
-  return row_bytes == 128 ? (r & 7) : (row_bytes == 64 ? ((r >> 1) & 3) : ((r >> 2) & 1));
 }
 
 constexpr int TC_CONSUMERS = 256;                // warps 0-7: two warpgroups, rows 0-63 / 64-127 of every tile
@@ -648,30 +601,28 @@ EncodeTiledFn tmap_encode_fn() {
 }
 
 int sm_count() {
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return num_sms;
+  static std::mutex mu;
+  static std::map<int, int> num_sms;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lock(mu);
+  int& n = num_sms[dev];
+  if (!n) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  return n;
 }
 
-// 4-D tensor map {C, W, H, N} of an fp16 NHWC buffer whose pixels are `pitch` channels apart, starting at channel coff
-static CUresult tmap_nhwc(CUtensorMap* map, void* base, int coff, int C, int W, int H, int N, int pitch, const cuuint32_t* box,
-                          const cuuint32_t* estr, CUtensorMapSwizzle swz) {
+CUresult tmap_nhwc(CUtensorMap* map, CUtensorMapDataType type, void* base, int coff, int C, int W, int H, int N, int pitch,
+                   const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapSwizzle swz) {
   const EncodeTiledFn encode = tmap_encode_fn();
   if (!encode) return CUDA_ERROR_NOT_FOUND;
+  const cuuint64_t esz = type == CU_TENSOR_MAP_DATA_TYPE_FLOAT32 ? 4 : 2;
   const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  const cuuint64_t gstr[3] = {(cuuint64_t)pitch * 2, (cuuint64_t)pitch * 2 * W, (cuuint64_t)pitch * 2 * W * H};
-  return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, static_cast<__half*>(base) + coff, gdim, gstr, box, estr,
-                CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const cuuint64_t gstr[3] = {pitch * esz, pitch * esz * W, pitch * esz * W * H};
+  return encode(map, type, 4, static_cast<uint8_t*>(base) + coff * esz, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
+                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-// Dynamic shared-memory limit of a kernel for a launch of `smem` bytes (and, for the persistent ring kernels, the
-// largest carveout).  Plans of different shapes share an instantiation: its limit (per device) only ever grows to the
-// largest plan made so far, so a smaller plan created later cannot make an earlier one's launch fail.
-static cudaError_t smem_limit(const void* kernel, size_t smem, bool max_carveout) {
+cudaError_t smem_limit(const void* kernel, size_t smem, bool max_carveout) {
   static std::mutex mu;
   static std::map<std::pair<int, const void*>, size_t> limit;
   int dev = 0;
@@ -827,7 +778,8 @@ TcConvPlan* tc_conv_plan_create(const ConvParams& p, std::string* err) {
     box[1] = a.BW * p.stride; box[2] = a.BH * p.stride;
     estr[1] = estr[2] = p.stride;
   }
-  const CUresult cr = tmap_nhwc(&a.tmA, p.in.base, p.in.coff, mC, mW, mH, mN, m_pitch, box, estr, row_swizzle(m_row_bytes));
+  const CUresult cr = tmap_nhwc(&a.tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, p.in.base, p.in.coff, mC, mW, mH, mN, m_pitch, box, estr,
+                                row_swizzle(m_row_bytes));
   if (cr != CUDA_SUCCESS) {
     if (err) *err = "cuTensorMapEncodeTiled(A) failed with code " + std::to_string((int)cr);
     return nullptr;
@@ -1267,8 +1219,8 @@ TcBneckPlan* tc_bneck_plan_create(const TcConvPlan* pa, const TcConvPlan* pb, st
   BnArgs& a = plan->args;
   memset(&a, 0, sizeof(a));
   const cuuint32_t box[4] = {(cuuint32_t)a1.BK, (cuuint32_t)BN_PITCH, (cuuint32_t)(HALO_BH + 4), 1}, estr[4] = {1, 1, 1, 1};
-  if (tmap_nhwc(&a.tmX, p1.in.base, p1.in.coff, p1.Cin, p1.in.W, p1.in.H, p1.B, p1.in.pitch, box, estr, row_swizzle(a1.BK * 2)) !=
-      CUDA_SUCCESS)
+  if (tmap_nhwc(&a.tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, p1.in.base, p1.in.coff, p1.Cin, p1.in.W, p1.in.H, p1.B, p1.in.pitch, box,
+                estr, row_swizzle(a1.BK * 2)) != CUDA_SUCCESS)
     return fail("cuTensorMapEncodeTiled(bottleneck input) failed");
   a.w1 = a1.wpk; a.w2 = a2.wpk;
   a.bias1 = p1.bias; a.bias2 = p2.bias;

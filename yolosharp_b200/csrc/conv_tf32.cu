@@ -39,12 +39,6 @@
 
 namespace yb {
 
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 constexpr int TF_MAX_STAGES = 8;
 constexpr int TF_CONSUMER_WARPS = 8;                      // two warpgroups (tf_conv_kernel) / eight MMA warps (wgrad)
 constexpr int TF_THREADS = 32 * TF_CONSUMER_WARPS + 32;  // + warp 8: TMA producer
@@ -56,13 +50,14 @@ constexpr int ST_WG_BLOCKS = 592;
 // ------------------------------------------------------------------------------------------
 struct TfArgs {
   CUtensorMap tmA, tmB;
+  TileGrid tg;
   float* out;
   const float* bias;                // [n_out] or nullptr
   long long o_img, o_row, o_pix;    // element strides of the output addressing
   long long o_off;
   int n_out;                        // valid output channels (columns >= n_out are not stored)
-  int Ho, Wo, imgs;                 // extent of the output position grid the tiles cover
-  int tiles_w, tiles_h, n_tiles, n_tile, total_tiles;
+  int Ho, Wo;                       // extent of the output position grid the tiles cover
+  int n_tile;
   int BW, BH;
   int in_stride;                    // A box origin = (w0 * in_stride + dw, h0 * in_stride + dh)
   int ntaps;
@@ -94,7 +89,7 @@ __device__ __forceinline__ void tf_mainloop(const TfArgs& a, float* acc, uint32_
     __syncwarp();
     if (leader && pend) mbar_arrive(pend);
     pend = empty0 + 8 * st;
-    if (++st == a.stages) { st = 0; ph ^= 1; }
+    ring_next(st, ph, a.stages);
   }
   wg_wait<0>();
   __syncwarp();
@@ -119,7 +114,6 @@ __global__ void __launch_bounds__(TF_THREADS, NT16 <= 4 ? 2 : 1) tf_conv_kernel(
   __syncthreads();
   pdl_wait();
   pdl_trigger();
-  const int tiles_per_img = a.tiles_w * a.tiles_h;
 
   if (warp == TF_CONSUMER_WARPS) {
     if (lane == 0) {
@@ -127,43 +121,39 @@ __global__ void __launch_bounds__(TF_THREADS, NT16 <= 4 ? 2 : 1) tf_conv_kernel(
       asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmB) : "memory");
       int st = 0;
       uint32_t ph = 0;
-      for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
-        const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-        const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
-        const int th = r / a.tiles_w, tw = r - th * a.tiles_w;
-        const int wbase = tw * a.BW * a.in_stride, hbase = th * a.BH * a.in_stride;
+      for (int tile = blockIdx.x; tile < a.tg.total; tile += gridDim.x) {
+        const TileCoord tc = tile_coord(a.tg, tile);
+        const int wbase = tc.tw * a.BW * a.in_stride, hbase = tc.th * a.BH * a.in_stride;
         for (int t = 0; t < a.ntaps; t++)
           for (int ch = 0; ch < a.chunks; ch++) {
             mbar_wait(empty0 + 8 * st, ph ^ 1);
             mbar_arrive_expect_tx(full0 + 8 * st, a.a_bytes + a.b_bytes);
-            tma_load_4d(smemA + st * a.a_stride, &a.tmA, full0 + 8 * st, ch * a.BK, wbase + a.dw[t], hbase + a.dh[t], img);
-            tma_load_3d(smemB + st * a.b_stride, &a.tmB, full0 + 8 * st, ch * a.BK, nt * a.n_tile, a.slab[t]);
-            if (++st == a.stages) { st = 0; ph ^= 1; }
+            tma_load_4d(smemA + st * a.a_stride, &a.tmA, full0 + 8 * st, ch * a.BK, wbase + a.dw[t], hbase + a.dh[t], tc.img);
+            tma_load_3d(smemB + st * a.b_stride, &a.tmB, full0 + 8 * st, ch * a.BK, tc.nt * a.n_tile, a.slab[t]);
+            ring_next(st, ph, a.stages);
           }
       }
     }
   } else {
-    const int wg = warp >> 2, g = lane >> 2, t4 = lane & 3;
+    const int t4 = lane & 3;
     int st = 0;
     uint32_t ph = 0;
-    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
+    for (int tile = blockIdx.x; tile < a.tg.total; tile += gridDim.x) {
       float acc[NT16 * 8];
       switch (a.KK) {
         case 4: tf_mainloop<NT16, 4>(a, acc, smemA, smemB, full0, empty0, st, ph); break;
         case 2: tf_mainloop<NT16, 2>(a, acc, smemA, smemB, full0, empty0, st, ph); break;
         default: tf_mainloop<NT16, 1>(a, acc, smemA, smemB, full0, empty0, st, ph); break;
       }
-      const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-      const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
-      const int th = r / a.tiles_w, tw = r - th * a.tiles_w;
-      const int n0 = nt * a.n_tile;
+      const TileCoord tc = tile_coord(a.tg, tile);
+      const int n0 = tc.nt * a.n_tile;
 #pragma unroll
       for (int h = 0; h < 2; h++) {
-        const int row = wg * 64 + (warp & 3) * 16 + g + 8 * h;
+        const int row = acc_row(warp >> 2, h);
         const int hl = row / a.BW, wl = row - hl * a.BW;
-        const int ho = th * a.BH + hl, wo = tw * a.BW + wl;
+        const int ho = tc.th * a.BH + hl, wo = tc.tw * a.BW + wl;
         if (hl >= a.BH || ho >= a.Ho || wo >= a.Wo) continue;
-        float* orow = a.out + (long long)img * a.o_img + (long long)ho * a.o_row + (long long)wo * a.o_pix + a.o_off + n0;
+        float* orow = a.out + (long long)tc.img * a.o_img + (long long)ho * a.o_row + (long long)wo * a.o_pix + a.o_off + n0;
 #pragma unroll
         for (int J = 0; J < NT16 * 2; J++) {
           const int c = 8 * J + 2 * t4;
@@ -259,27 +249,24 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
   a.chunks = (L.Kc + a.BK - 1) / a.BK;
   a.KK = a.BK / 8;
   const uint32_t row_bytes = a.BK * 4;
-  a.layout = a.BK == 32 ? 1 : (a.BK == 16 ? 2 : 3);
+  a.layout = row_layout(row_bytes);
   a.sbo16 = (8 * row_bytes) >> 4;
-  const CUtensorMapSwizzle swz = a.BK == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : (a.BK == 16 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+  const CUtensorMapSwizzle swz = row_swizzle(row_bytes);
   a.n_tile = std::min(256, (L.Nc + 15) / 16 * 16);
-  a.n_tiles = (L.Nc + a.n_tile - 1) / a.n_tile;
+  const int n_tiles = (L.Nc + a.n_tile - 1) / a.n_tile;
   // One N tile as wide as the layer: narrower tiles would give every SM a tile on the 20 x 20 / 40 x 40 levels, at the price
   // of re-reading the activations once per N tile.
-  cuuint64_t gdim[4], gstr[3];
+  // The flat map is the NHWC map of one image of 1 x (N * H * W) pixels.
+  const int npix = L.N * L.Hi * L.Wi;
+  const int imgs = L.flat ? 1 : L.N, Hi = L.flat ? 1 : L.Hi, Wi = L.flat ? npix : L.Wi;
   cuuint32_t box[4], estr[4];
   if (L.flat) {
-    const cuuint64_t npix = (cuuint64_t)L.N * L.Hi * L.Wi;
-    gdim[0] = L.Kc; gdim[1] = npix; gdim[2] = 1; gdim[3] = 1;
-    gstr[0] = (cuuint64_t)(L.in_pitch ? L.in_pitch : L.Kc) * 4; gstr[1] = gstr[0] * npix; gstr[2] = gstr[1];
     a.BW = 128; a.BH = 1;
-    a.imgs = 1; a.Ho = 1; a.Wo = (int)npix;
+    a.Ho = 1; a.Wo = npix;
     box[0] = a.BK; box[1] = 128; box[2] = 1; box[3] = 1;
     estr[0] = estr[1] = estr[2] = estr[3] = 1;
   } else {
-    gdim[0] = L.Kc; gdim[1] = L.Wi; gdim[2] = L.Hi; gdim[3] = L.N;
-    gstr[0] = (cuuint64_t)(L.in_pitch ? L.in_pitch : L.Kc) * 4; gstr[1] = gstr[0] * L.Wi; gstr[2] = gstr[1] * L.Hi;
-    a.imgs = L.N; a.Ho = L.Ho; a.Wo = L.Wo;
+    a.Ho = L.Ho; a.Wo = L.Wo;
     double best = -1;
     for (int bw = 1; bw <= std::min(L.Wo, 128); bw++) {
       const int bh = std::min(L.Ho, 128 / bw);
@@ -291,8 +278,8 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
     box[0] = a.BK; box[1] = a.BW * L.in_stride; box[2] = a.BH * L.in_stride; box[3] = 1;
     estr[0] = 1; estr[1] = L.in_stride; estr[2] = L.in_stride; estr[3] = 1;
   }
-  CUresult cr = encode(&a.tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(L.in), gdim, gstr, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult cr = tmap_nhwc(&a.tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, const_cast<float*>(L.in), 0, L.Kc, Wi, Hi, imgs,
+                          L.in_pitch ? L.in_pitch : L.Kc, box, estr, swz);
   if (cr != CUDA_SUCCESS) { set_error("tf32 conv: cuTensorMapEncodeTiled(A) failed with code " + std::to_string((int)cr)); return YB_ERR_CUDA; }
   {
     cuuint64_t bd[3] = {(cuuint64_t)L.Kc, (cuuint64_t)L.Nc, (cuuint64_t)L.taps_total};
@@ -303,9 +290,7 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) { set_error("tf32 conv: cuTensorMapEncodeTiled(B) failed with code " + std::to_string((int)cr)); return YB_ERR_CUDA; }
   }
-  a.tiles_w = (a.Wo + a.BW - 1) / a.BW;
-  a.tiles_h = (a.Ho + a.BH - 1) / a.BH;
-  a.total_tiles = a.imgs * a.tiles_w * a.tiles_h * a.n_tiles;
+  a.tg = tile_grid(imgs, a.Ho, a.Wo, a.BH, a.BW, n_tiles);
   a.a_bytes = (uint32_t)(a.BW * a.BH) * row_bytes;  // the box has BW*BH <= 128 rows; rows past it are never stored
   a.b_bytes = (uint32_t)a.n_tile * row_bytes;
   a.a_stride = (128 * row_bytes + 1023) / 1024 * 1024;
@@ -315,22 +300,18 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
   // the other's load -> MMA -> epilogue bubbles, as in conv_tc_kernel.
   const size_t per_stage = (size_t)a.a_stride + a.b_stride;
   int occ = 1;
-  if (a.n_tile <= 64 && (size_t)(100 * 1024) / per_stage >= 3 && a.total_tiles >= 2 * sm_count()) occ = 2;
+  if (a.n_tile <= 64 && (size_t)(100 * 1024) / per_stage >= 3 && a.tg.total >= 2 * sm_count()) occ = 2;
   a.stages = (int)std::min<size_t>(TF_MAX_STAGES, (size_t)((occ == 2 ? 100 : 190) * 1024) / per_stage);
   if (a.stages < 2) { set_error("tf32 conv: tile does not fit in shared memory"); return YB_ERR_SHAPE; }
   const size_t smem = (size_t)a.stages * (a.a_stride + a.b_stride) + 1024;
   void (*kernel)(TfArgs) = nullptr;
   dispatch_nt16(a.n_tile / 16, [&](auto nt16) { kernel = tf_conv_kernel<decltype(nt16)::value>; });
-  static bool attr_set[17] = {};
-  if (!attr_set[a.n_tile / 16]) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set[a.n_tile / 16] = true;
-  }
-  const int grid = std::min(a.total_tiles, occ * sm_count());
+  YB_CUDA_CHECK(smem_limit((const void*)kernel, smem, false));
+  const int grid = std::min(a.tg.total, occ * sm_count());
   if (desc) {
     char line[256];
     snprintf(line, sizeof(line), "%stf_conv_kernel BK %d chunks %d n_tile %d x%d BW %d BH %d in_stride %d flat %d ntaps %d occ %d stages %d grid %d",
-             desc->empty() ? "" : "\n", a.BK, a.chunks, a.n_tile, a.n_tiles, a.BW, a.BH, a.in_stride, L.flat ? 1 : 0, a.ntaps, occ,
+             desc->empty() ? "" : "\n", a.BK, a.chunks, a.n_tile, a.tg.n_tiles, a.BW, a.BH, a.in_stride, L.flat ? 1 : 0, a.ntaps, occ,
              a.stages, grid);
     *desc += line;
   }
@@ -433,7 +414,7 @@ struct WgArgs {
   int co_blocks;    // 32-channel output blocks loaded per CTA (<= 4)
   int co_tiles, ci_tiles, splits;
   int tpc, tap_groups;  // taps per CTA (3 = one kh row of a 3x3, 1 for 1x1) and groups of them
-  int imgs, tiles_w, tiles_h, pix_tiles;
+  TileGrid tg;       // pixel tiles of the dz grid (n_tiles = 1)
   int b_stages;
   int halo;         // 3x3 stride 1: ONE PH x (PW+2) input tile per pixel tile serves the three taps of a kh row (row-shifted windows)
   uint32_t xblk;    // bytes reserved per 32-channel block of an x stage (1 KiB aligned)
@@ -481,8 +462,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_wgrad_kernel(const __grid_co
   const int tg = rest % a.tap_groups, pair = rest / a.tap_groups;
   const int ci_t = pair % a.ci_tiles, co_t = pair / a.ci_tiles;
   const int tap0 = tg * a.tpc;
-  const int tiles_per_img = a.tiles_w * a.tiles_h;
-  const int my_tiles = split < a.pix_tiles ? (a.pix_tiles - split + a.splits - 1) / a.splits : 0;
+  const int my_tiles = split < a.tg.total ? (a.tg.total - split + a.splits - 1) / a.splits : 0;
   const int ncols = a.nb * 32;  // accumulator columns per tap
 
   if (warp == TF_CONSUMER_WARPS) {
@@ -492,15 +472,13 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_wgrad_kernel(const __grid_co
       int sa = 0, sb = 0;
       uint32_t pa = 0, pb = 0;
       for (int i = 0; i < my_tiles; i++) {
-        const int pt = split + i * a.splits;
-        const int img = pt / tiles_per_img, r = pt - img * tiles_per_img;
-        const int th = r / a.tiles_w, tw = r - th * a.tiles_w;
-        const int w0 = tw * WG_PW, h0 = th * WG_PH;
+        const TileCoord tc = tile_coord(a.tg, split + i * a.splits);
+        const int w0 = tc.tw * WG_PW, h0 = tc.th * WG_PH;
         mbar_wait(aempty + 8 * sa, pa ^ 1);
         mbar_arrive_expect_tx(afull + 8 * sa, (uint32_t)a.co_blocks * WG_BLK);
         for (int b = 0; b < a.co_blocks; b++)
-          tma_load_4d(smemA + sa * a_stride + b * WG_BLK, &a.tmDz, afull + 8 * sa, co_t * 128 + b * 32, w0, h0, img);
-        if (++sa == WG_A_STAGES) { sa = 0; pa ^= 1; }
+          tma_load_4d(smemA + sa * a_stride + b * WG_BLK, &a.tmDz, afull + 8 * sa, co_t * 128 + b * 32, w0, h0, tc.img);
+        ring_next(sa, pa, WG_A_STAGES);
         if (a.halo) {
           // one box of PH x (PW + 2) input pixels per 32-channel block for the kh row of this CTA: tap (kh, kw) of output
           // row h reads its 8 pixels from rows h * (PW + 2) + kw .. + 7 of it
@@ -508,8 +486,8 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_wgrad_kernel(const __grid_co
           mbar_wait(bempty + 8 * sb, pb ^ 1);
           mbar_arrive_expect_tx(bfull + 8 * sb, (uint32_t)a.nb * (WG_PW + 2) * WG_PH * 128);
           for (int b = 0; b < a.nb; b++)
-            tma_load_4d(smemB + sb * b_stride + b * a.xblk, &a.tmX, bfull + 8 * sb, (ci_t * a.nb + b) * 32, w0 - a.pad, h0 + kh - a.pad, img);
-          if (++sb == a.b_stages) { sb = 0; pb ^= 1; }
+            tma_load_4d(smemB + sb * b_stride + b * a.xblk, &a.tmX, bfull + 8 * sb, (ci_t * a.nb + b) * 32, w0 - a.pad, h0 + kh - a.pad, tc.img);
+          ring_next(sb, pb, a.b_stages);
         } else {
           for (int tt = 0; tt < a.tpc; tt++) {
             const int t = tap0 + tt;
@@ -518,8 +496,8 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_wgrad_kernel(const __grid_co
             mbar_arrive_expect_tx(bfull + 8 * sb, (uint32_t)a.nb * WG_BLK);
             for (int b = 0; b < a.nb; b++)
               tma_load_4d(smemB + sb * b_stride + b * a.xblk, &a.tmX, bfull + 8 * sb, (ci_t * a.nb + b) * 32,
-                          w0 * a.stride + kw - a.pad, h0 * a.stride + kh - a.pad, img);
-            if (++sb == a.b_stages) { sb = 0; pb ^= 1; }
+                          w0 * a.stride + kw - a.pad, h0 * a.stride + kh - a.pad, tc.img);
+            ring_next(sb, pb, a.b_stages);
           }
         }
       }
@@ -569,9 +547,8 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_wgrad_kernel(const __grid_co
         mbar_arrive(aempty + 8 * sa);
         for (int q = 0; q < nst; q++) mbar_arrive(bempty + 8 * (sb + q < a.b_stages ? sb + q : sb + q - a.b_stages));
       }
-      if (++sa == WG_A_STAGES) { sa = 0; pa ^= 1; }
-      for (int q = 0; q < nst; q++)
-        if (++sb == a.b_stages) { sb = 0; pb ^= 1; }
+      ring_next(sa, pa, WG_A_STAGES);
+      for (int q = 0; q < nst; q++) ring_next(sb, pb, a.b_stages);
     }
 #pragma unroll
     for (int h = 0; h < 2; h++) {
@@ -619,7 +596,7 @@ __global__ void __launch_bounds__(256) tf_wgrad_fold_kernel(const float* __restr
   for (int e = threadIdx.x; e < n; e += 256) out[e] = fold_sm[e];
 }
 
-struct WgPlan { int nb, co_tiles, ci_tiles, splits, co_pad, ci_pad, pix_tiles, tiles_w, tiles_h, tpc, tap_groups; };
+struct WgPlan { int nb, co_tiles, ci_tiles, splits, co_pad, ci_pad, tpc, tap_groups; TileGrid tg; };
 static WgPlan wg_plan(int N, int H, int W, int Cin, int Cout, int k, int stride, int pad) {
   WgPlan p;
   const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
@@ -633,9 +610,7 @@ static WgPlan wg_plan(int N, int H, int W, int Cin, int Cout, int k, int stride,
   p.co_tiles = (Cout + 127) / 128;
   p.co_pad = p.co_tiles * 128;
   p.ci_pad = p.ci_tiles * p.nb * 32;
-  p.tiles_w = (Wo + WG_PW - 1) / WG_PW;
-  p.tiles_h = (Ho + WG_PH - 1) / WG_PH;
-  p.pix_tiles = N * p.tiles_w * p.tiles_h;
+  p.tg = tile_grid(N, Ho, Wo, WG_PH, WG_PW, 1);
   p.tap_groups = taps / p.tpc;
   const int pairs = p.co_tiles * p.ci_tiles * p.tap_groups;
   // pixel splits: one CTA per SM (189 KiB of shared memory), so the grid should fill ONE wave of SMs, or two when that fills
@@ -645,7 +620,7 @@ static WgPlan wg_plan(int N, int H, int W, int Cin, int Cout, int k, int stride,
   const int s1 = std::max(1, sms / pairs), s2 = std::max(1, 2 * sms / pairs);
   const double u1 = (double)std::min(pairs * s1, sms) / sms, u2 = (double)std::min(pairs * s2, 2 * sms) / (2.0 * sms);
   p.splits = (pairs <= sms && u2 > u1 + 0.08) ? s2 : s1;
-  p.splits = std::max(1, std::min(p.splits, p.pix_tiles));
+  p.splits = std::max(1, std::min(p.splits, p.tg.total));
   return p;
 }
 
@@ -661,8 +636,7 @@ int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W
   if (x_pitch && (x_pitch < Cin || x_pitch % 4 || ((uintptr_t)x & 15))) { set_error("tf32 wgrad: input view must be 16-byte aligned with a pitch multiple of 4"); return YB_ERR_SHAPE; }
   const int xp = x_pitch ? x_pitch : Cin;
   if (!tf_shape_ok(Cin, Cout, k, stride, pad)) { set_error("tf32 wgrad: channels must be multiples of 8, k in {1,3}, stride in {1,2}, pad = k/2"); return YB_ERR_SHAPE; }
-  const EncodeTiledFn encode = tmap_encode_fn();
-  if (!encode) { set_error("cuTensorMapEncodeTiled entry point not found"); return YB_ERR_CUDA; }
+  if (!tmap_encode_fn()) { set_error("cuTensorMapEncodeTiled entry point not found"); return YB_ERR_CUDA; }
   const WgPlan p = wg_plan(N, H, W, Cin, Cout, k, stride, pad);
   const size_t part_bytes = (size_t)p.splits * p.co_pad * k * k * p.ci_pad * 4;
   if (ws_bytes < part_bytes) { set_error("tf32 wgrad: workspace too small"); return YB_ERR_INVALID_ARG; }
@@ -674,7 +648,7 @@ int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W
   a.nb = p.nb; a.co_tiles = p.co_tiles; a.ci_tiles = p.ci_tiles; a.splits = p.splits;
   a.tpc = p.tpc; a.tap_groups = p.tap_groups;
   a.co_blocks = std::min(4, (Cout + 31) / 32);
-  a.imgs = N; a.tiles_w = p.tiles_w; a.tiles_h = p.tiles_h; a.pix_tiles = p.pix_tiles;
+  a.tg = p.tg;
   a.co_pad = p.co_pad; a.ci_pad = p.ci_pad;
   // 3x3 stride 1: the input tile with its halo is loaded once per pixel tile and the nine taps are row-shifted MMA windows
   // into it (the per-tap form moved 9 x 8 KiB of x per 64 pixels and was bound by L2 -> SM delivery).
@@ -684,47 +658,33 @@ int tf_conv_backward_weight(const float* x, const float* dz, int N, int H, int W
   a.b_stages = (int)std::min<size_t>(16, ((size_t)190 * 1024 - (size_t)WG_A_STAGES * 4 * WG_BLK) / b_stride);
   if (a.b_stages < 2) { set_error("tf32 wgrad: tile does not fit in shared memory"); return YB_ERR_SHAPE; }
   {
-    cuuint64_t gd[4] = {(cuuint64_t)Cout, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)N};
-    cuuint64_t gs[3] = {(cuuint64_t)Cout * 4, (cuuint64_t)Cout * 4 * Wo, (cuuint64_t)Cout * 4 * Wo * Ho};
-    cuuint32_t bx[4] = {32, WG_PW, WG_PH, 1};
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    CUresult cr = encode(&a.tmDz, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(dz), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint32_t bx[4] = {32, WG_PW, WG_PH, 1}, es[4] = {1, 1, 1, 1};
+    const CUresult cr = tmap_nhwc(&a.tmDz, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, const_cast<float*>(dz), 0, Cout, Wo, Ho, N, Cout, bx, es,
+                                  CU_TENSOR_MAP_SWIZZLE_128B);
     if (cr != CUDA_SUCCESS) { set_error("tf32 wgrad: cuTensorMapEncodeTiled(dz) failed with code " + std::to_string((int)cr)); return YB_ERR_CUDA; }
   }
   {
-    cuuint64_t gd[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-    cuuint64_t gs[3] = {(cuuint64_t)xp * 4, (cuuint64_t)xp * 4 * W, (cuuint64_t)xp * 4 * W * H};
-    cuuint32_t bx[4] = {32, (cuuint32_t)(a.halo ? WG_PW + 2 : WG_PW * stride), (cuuint32_t)(a.halo ? WG_PH : WG_PH * stride), 1};
-    cuuint32_t es[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-    CUresult cr = encode(&a.tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint32_t bx[4] = {32, (cuuint32_t)(a.halo ? WG_PW + 2 : WG_PW * stride), (cuuint32_t)(a.halo ? WG_PH : WG_PH * stride), 1};
+    const cuuint32_t es[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+    const CUresult cr = tmap_nhwc(&a.tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, const_cast<float*>(x), 0, Cin, W, H, N, xp, bx, es,
+                                  CU_TENSOR_MAP_SWIZZLE_128B);
     if (cr != CUDA_SUCCESS) { set_error("tf32 wgrad: cuTensorMapEncodeTiled(x) failed with code " + std::to_string((int)cr)); return YB_ERR_CUDA; }
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(tf_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set = true;
-  }
   const size_t smem = (size_t)WG_A_STAGES * 4 * WG_BLK + (size_t)a.b_stages * b_stride + 1024;
+  YB_CUDA_CHECK(smem_limit((const void*)tf_wgrad_kernel, smem, false));
   const int grid = p.co_tiles * p.ci_tiles * p.tap_groups * p.splits;
   if (desc) {
     char line[256];
     snprintf(line, sizeof(line), "%stf_wgrad_kernel halo %d tpc %d nb %d co_tiles %d ci_tiles %d co_blocks %d splits %d pix_tiles %d b_stages %d grid %d",
-             desc->empty() ? "" : "\n", a.halo, a.tpc, a.nb, a.co_tiles, a.ci_tiles, a.co_blocks, a.splits, a.pix_tiles, a.b_stages, grid);
+             desc->empty() ? "" : "\n", a.halo, a.tpc, a.nb, a.co_tiles, a.ci_tiles, a.co_blocks, a.splits, a.tg.total, a.b_stages, grid);
     *desc += line;
   }
   YB_CUDA_CHECK(launch_pdl(tf_wgrad_kernel, dim3(grid), dim3(TF_THREADS), smem, s, a));
-  const size_t n = (size_t)Cout * Cin * k * k;
-  static bool fold_attr = false;
-  if (!fold_attr) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(tf_wgrad_fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    fold_attr = true;
-  }
-  if ((size_t)Cin * k * k * sizeof(float) > (size_t)160 * 1024) { set_error("tf32 wgrad: Cin * k * k too large for the fold"); return YB_ERR_SHAPE; }
-  YB_CUDA_CHECK(launch_pdl(tf_wgrad_fold_kernel, dim3(Cout), dim3(256), (size_t)Cin * k * k * sizeof(float), s, (const float*)ws, dw, Cout, Cin, k * k,
+  const size_t fold_smem = (size_t)Cin * k * k * sizeof(float);
+  if (fold_smem > (size_t)160 * 1024) { set_error("tf32 wgrad: Cin * k * k too large for the fold"); return YB_ERR_SHAPE; }
+  YB_CUDA_CHECK(smem_limit((const void*)tf_wgrad_fold_kernel, fold_smem, false));
+  YB_CUDA_CHECK(launch_pdl(tf_wgrad_fold_kernel, dim3(Cout), dim3(256), fold_smem, s, (const float*)ws, dw, Cout, Cin, k * k,
                            p.splits, p.co_pad, p.ci_pad));
-  (void)n;
   YB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -898,20 +858,11 @@ int stem3_backward_weight(const float* x, int xc, const float* dz, int N, int H,
   if (ws_bytes < stem3_wgrad_workspace_bytes(C)) { set_error("stem wgrad: workspace too small"); return YB_ERR_INVALID_ARG; }
   const int Ho = H / 2, Wo = W / 2;
   const size_t smem = (size_t)(3 * (2 * ST_PIX + 1) * 4 + std::max(ST_PIX * C, 8 * 27 * 32)) * sizeof(float);
-  static bool attr = false;
-  if (!attr) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(stem3_wgrad_partial_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    YB_CUDA_CHECK(cudaFuncSetAttribute(stem3_wgrad_partial_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    YB_CUDA_CHECK(cudaFuncSetAttribute(stem3_wgrad_partial_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    YB_CUDA_CHECK(cudaFuncSetAttribute(stem3_wgrad_partial_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    attr = true;
-  }
-  switch ((C + 31) / 32) {
-    case 1: stem3_wgrad_partial_kernel<1><<<blocks, 256, smem, s>>>(x, xc, dz, ws, N, H, W, Ho, Wo, C); break;
-    case 2: stem3_wgrad_partial_kernel<2><<<blocks, 256, smem, s>>>(x, xc, dz, ws, N, H, W, Ho, Wo, C); break;
-    case 3: stem3_wgrad_partial_kernel<3><<<blocks, 256, smem, s>>>(x, xc, dz, ws, N, H, W, Ho, Wo, C); break;
-    default: stem3_wgrad_partial_kernel<4><<<blocks, 256, smem, s>>>(x, xc, dz, ws, N, H, W, Ho, Wo, C); break;
-  }
+  const int cg = (C + 31) / 32;
+  const auto kernel = cg == 1 ? stem3_wgrad_partial_kernel<1> : cg == 2 ? stem3_wgrad_partial_kernel<2>
+                    : cg == 3 ? stem3_wgrad_partial_kernel<3> : stem3_wgrad_partial_kernel<4>;
+  YB_CUDA_CHECK(smem_limit((const void*)kernel, smem, false));
+  kernel<<<blocks, 256, smem, s>>>(x, xc, dz, ws, N, H, W, Ho, Wo, C);
   stem3_wgrad_fold_kernel<<<(27 * C + 127) / 128, 128, 0, s>>>(ws, blocks, C, dw);
   YB_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -925,8 +876,7 @@ extern "C" {
 
 int64_t yb_conv_tc_workspace_bytes(int32_t n, int32_t height, int32_t width, int32_t cin, int32_t cout, int32_t k, int32_t stride) {
   if (n <= 0 || height <= 0 || width <= 0 || cin <= 0 || cout <= 0 || k <= 0 || stride <= 0) return 0;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return 0; }
+  if (!have_device("yb_conv_tc_workspace_bytes")) return 0;
   return (int64_t)tf_conv_workspace_bytes(n, height, width, cin, cout, k, stride);
 }
 

@@ -796,13 +796,14 @@ static int run_ops(yb_engine* e, const void* in, int in_dtype, int B, float* out
   return 0;
 }
 
-bool have_device(const char* who) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+bool have_device(const char* who, int* ndev) {
+  int n = 0;
+  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
     cudaGetLastError();
-    set_error(std::string(who) + ": no CUDA device");
+    set_error(std::string(who) + ": no CUDA device (this library has no CPU fallback)");
     return false;
   }
+  if (ndev) *ndev = n;
   return true;
 }
 
@@ -841,11 +842,7 @@ int32_t yb_create(const yb_config* cfg, yb_engine** out) {
     return YB_OK;
   }
   int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error("yb_create: no CUDA device available (this engine has no CPU fallback)");
-    return YB_ERR_NO_DEVICE;
-  }
+  if (!have_device("yb_create", &ndev)) return YB_ERR_NO_DEVICE;
   if (cfg->device < 0 || cfg->device >= ndev) { set_error("yb_create: bad device ordinal"); return YB_ERR_INVALID_ARG; }
   YB_CUDA_CHECK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
@@ -1163,12 +1160,7 @@ int32_t yb_detection_loss(const float* boxes, const float* scores, int32_t batch
     set_error("yb_detection_loss: null argument");
     return YB_ERR_INVALID_ARG;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error("yb_detection_loss: no CUDA device");
-    return YB_ERR_NO_DEVICE;
-  }
+  if (!have_device("yb_detection_loss")) return YB_ERR_NO_DEVICE;
   return detection_loss_launch(boxes, scores, batch, nc, reg_max, height, width, targets_host, n_targets, topk, hyp_box,
                                hyp_cls, hyp_dfl, loss_items, grad_boxes, grad_scores, fg, gt_idx, target_score,
                                (cudaStream_t)stream);

@@ -382,13 +382,7 @@ int launch_sppf_pool(const View& in, const View& o5, const View& o9, const View&
     set_error("sppf_pool: feature map too large for the shared-memory kernel");
     return YB_ERR_SHAPE;
   }
-  static bool attr_set[2] = {false, false};
-  const int ti = sizeof(T) == 4 ? 0 : 1;
-  if (!attr_set[ti] && smem > 48 * 1024) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(sppf_pool_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       200 * 1024));
-    attr_set[ti] = true;
-  }
+  YB_CUDA_CHECK(smem_limit((const void*)sppf_pool_kernel<T>, smem, false));
   dim3 grid((in.C + SP_CC - 1) / SP_CC, B);
   sppf_pool_kernel<T><<<grid, 256, smem, s>>>(in, o5, o9, o13);
   YB_CUDA_CHECK(cudaGetLastError());

@@ -356,8 +356,7 @@ int32_t yb_ap_per_class(const uint8_t* tp, const float* conf, const int32_t* pre
     set_error("yb_ap_per_class: null argument");
     return YB_ERR_INVALID_ARG;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); set_error("yb_ap_per_class: no CUDA device"); return YB_ERR_NO_DEVICE; }
+  if (!have_device("yb_ap_per_class")) return YB_ERR_NO_DEVICE;
   const int T = n_thresholds;
   int n2 = 1024;
   while (n2 < n) n2 <<= 1;

@@ -500,11 +500,7 @@ int nms_launch(const float* pred, int B, int C, int A, int nc, float conf, float
     pool_set = true;
   }
   YB_CUDA_CHECK(cudaMallocAsync(&gkeys, (size_t)B * P2 * 8, s));
-  static bool attr_set = false;
-  if (!attr_set) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NMS_TOTAL_SMEM));
-    attr_set = true;
-  }
+  YB_CUDA_CHECK(smem_limit((const void*)nms_kernel, smem, false));
   float* sconf = nullptr;
   YB_CUDA_CHECK(cudaMallocAsync(&sconf, (size_t)B * A * 8, s));  // conf[B][A] then cls[B][A]
   int* scls = reinterpret_cast<int*>(sconf + (size_t)B * A);
@@ -599,11 +595,7 @@ int masks_launch(const float* proto, const float* dets, const int* counts, int B
     set_error("yb_masks: proto map too large");
     return YB_ERR_SHAPE;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    YB_CUDA_CHECK(cudaFuncSetAttribute(masks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set = true;
-  }
+  YB_CUDA_CHECK(smem_limit((const void*)masks_kernel, smem, false));
   if (mask_cap <= 0 || mask_cap > max_det) mask_cap = max_det;
   masks_kernel<<<dim3(mask_cap, B), 512, smem, s>>>(proto, dets, counts, max_det, mask_cap, nm, mh, mw, H, W, masks);
   YB_CUDA_CHECK(cudaGetLastError());

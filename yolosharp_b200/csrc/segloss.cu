@@ -219,8 +219,7 @@ extern "C" int32_t yb_segmentation_loss(const uint8_t* fg, const int32_t* gt_idx
     set_error("yb_segmentation_loss: need 0 < nm <= 64 and positive sizes");
     return YB_ERR_SHAPE;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); set_error("yb_segmentation_loss: no CUDA device"); return YB_ERR_NO_DEVICE; }
+  if (!have_device("yb_segmentation_loss")) return YB_ERR_NO_DEVICE;
   const size_t BA = (size_t)batch * anchors;
   // scratch: list (int) | counts (int) | total (int) | cbox (6 f) | ccoef (nm f) | lossbuf (f)
   const size_t bytes = BA * 4 + (size_t)batch * 4 + 16 + BA * 6 * 4 + BA * nm * 4 + BA * 4 + 64;

@@ -45,6 +45,12 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -67,6 +73,52 @@ __device__ __forceinline__ int4 ld_shared_v4(uint32_t addr) {
 }
 
 // ------------------------------------------------------------------------------------------
+// Tile schedule, rings and operand rows shared by the fp16 (conv_tc.cu) and TF32 (conv_tf32.cu) convolutions
+// ------------------------------------------------------------------------------------------
+// exact x / d for x*d < 2^40 as (x * ceil(2^40/d)) >> 40 (runtime integer division costs ~100+ cycles)
+__device__ __forceinline__ int fdiv(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
+// the host side of fdiv: ceil(2^40 / d)
+inline uint64_t fdiv_magic(int d) { return (uint64_t)(((((unsigned __int128)1) << 40) + d - 1) / (unsigned)d); }
+
+// The tiles of one launch: `imgs` images of tiles_h x tiles_w output rectangles, each split into n_tiles N tiles.  Tile
+// index = ((img * tiles_h + th) * tiles_w + tw) * n_tiles + nt; the magic numbers divide by n_tiles, tpi and tiles_w.
+struct TileGrid {
+  int tiles_w, tpi, n_tiles, total;  // tpi = tiles per image
+  uint64_t m_ntiles, m_tpi, m_tw;
+};
+inline TileGrid tile_grid(int imgs, int H, int W, int BH, int BW, int n_tiles) {
+  TileGrid g;
+  g.tiles_w = (W + BW - 1) / BW;
+  g.tpi = g.tiles_w * ((H + BH - 1) / BH);
+  g.n_tiles = n_tiles;
+  g.total = imgs * g.tpi * n_tiles;
+  g.m_ntiles = fdiv_magic(n_tiles); g.m_tpi = fdiv_magic(g.tpi); g.m_tw = fdiv_magic(g.tiles_w);
+  return g;
+}
+struct TileCoord { int img, th, tw, nt; };
+__device__ __forceinline__ TileCoord tile_coord(const TileGrid& g, int tile) {
+  const int mt = fdiv(tile, g.m_ntiles);
+  const int img = fdiv(mt, g.m_tpi), r = mt - img * g.tpi;
+  const int th = fdiv(r, g.m_tw);
+  return {img, th, r - th * g.tiles_w, tile - mt * g.n_tiles};
+}
+
+// Next slot of an n-slot mbarrier ring; the wait parity flips on every wrap
+__device__ __forceinline__ void ring_next(int& s, uint32_t& ph, int n) {
+  if (++s == n) { s = 0; ph ^= 1; }
+}
+
+// Operand rows of 128 / 64 / 32 bytes: the tensor-map swizzle, the wgmma layout type it produces, and (device) the
+// 16-byte piece index XOR of row r under it
+inline CUtensorMapSwizzle row_swizzle(int row_bytes) {
+  return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+}
+inline uint32_t row_layout(int row_bytes) { return row_bytes == 128 ? 1 : (row_bytes == 64 ? 2 : 3); }
+__device__ __forceinline__ uint32_t row_swizzle_xor(uint32_t r, uint32_t row_bytes) {
+  return row_bytes == 128 ? (r & 7) : (row_bytes == 64 ? ((r >> 1) & 3) : ((r >> 2) & 1));
+}
+
+// ------------------------------------------------------------------------------------------
 // wgmma.  A warpgroup (4 consecutive warps, the first one's index a multiple of 4) computes a 64 x N tile; thread
 // (warp w of the group, lane l) holds rows 16w + l/4 and 16w + l/4 + 8, columns 8j + 2(l%4) + {0, 1}:
 //   d[4j + 0], d[4j + 1] = row 16w + l/4,     d[4j + 2], d[4j + 3] = row 16w + l/4 + 8.
@@ -82,6 +134,10 @@ template <int R>
 __device__ __forceinline__ void wg_fence_acc(float* d) {
 #pragma unroll
   for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Row of accumulator half h of this thread in m64 block `blk` of a tile (the D fragment above)
+__device__ __forceinline__ int acc_row(int blk, int h) {
+  return blk * 64 + ((threadIdx.x >> 5) & 3) * 16 + ((threadIdx.x & 31) >> 2) + 8 * h;
 }
 
 // Shared-memory matrix descriptor, K-major operand with swizzled rows, as two 32-bit words:

@@ -193,11 +193,6 @@ using namespace yb;
 extern "C" int32_t yb_topk_postprocess(const float* pred, int32_t batch, int32_t channels, int32_t anchors, int32_t nc,
                                        int32_t max_det, int32_t agnostic, float* out, int32_t* idx, void* stream) {
   if (!pred || !out || batch <= 0 || anchors <= 0) { set_error("yb_topk_postprocess: bad argument"); return YB_ERR_INVALID_ARG; }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error("yb_topk_postprocess: no CUDA device");
-    return YB_ERR_NO_DEVICE;
-  }
+  if (!have_device("yb_topk_postprocess")) return YB_ERR_NO_DEVICE;
   return topk_postprocess_launch(pred, batch, channels, anchors, nc, max_det, agnostic, out, idx, (cudaStream_t)stream);
 }

@@ -931,16 +931,6 @@ size_t max_workspace(yb_trainer* t) {
   return sw.ws + 4096;
 }
 
-bool have_dev(const char* who) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error(std::string(who) + ": no CUDA device");
-    return false;
-  }
-  return true;
-}
-
 // forward + loss + backward of one batch; gradients land in the caller's flat buffer
 int run_backward(yb_trainer* t, const void* images, int in_dtype, int B, const float* targets_host, int n_targets, float* items_host,
                  cudaStream_t s) {
@@ -1089,7 +1079,7 @@ int32_t yb_trainer_create(const yb_config* cfg, yb_trainer** out) {
   t->net.W = cfg->width;
   if (int rc = build(t.get(), cfg->arch, cfg->size, cfg->nc)) return rc;
   if (cfg->flags & YB_FLAG_DRY_RUN) { *out = t.release(); return YB_OK; }  // names / layout only (CPU tests)
-  if (!have_dev("yb_trainer_create")) return YB_ERR_NO_DEVICE;
+  if (!have_device("yb_trainer_create")) return YB_ERR_NO_DEVICE;
   if (cudaSetDevice(cfg->device) != cudaSuccess) { set_error("yb_trainer_create: cudaSetDevice failed"); cudaGetLastError(); return YB_ERR_CUDA; }
   {
     // the kernels' scratch (BatchNorm partials, attention statistics, ...) comes from the stream-ordered allocator; by
