@@ -266,7 +266,17 @@ int32_t yb_stem_conv_backward_weight_f32(const float* x, int32_t x_channels, con
  *                       BatchNorm ticket counters belong to the step in flight).
  *   yb_train_apply      one AdamW step (betas 0.9 / 0.999, eps 1e-8) with the two group learning rates
  *   yb_train_step       = yb_train_backward + yb_train_apply (single device)
- *   yb_get_grad / yb_get_tensor  copy one named gradient / parameter / running statistic to the host */
+ *   yb_get_grad / yb_get_tensor  copy one named gradient / parameter / running statistic to the host
+ *   yb_trainer_evaluate `AMPWrapper.Evaluate` (Utils/Amp.cs:387-395: the training model in `eval()`, its prediction
+ *                       `inference["boxes"]` and the raw head outputs `preds`): an eval-mode forward of the trainer's own
+ *                       graph at its current parameters and running statistics, in the training arithmetic (TF32
+ *                       tensor-core convolutions, fp32 storage).  BatchNorm uses the running statistics, folded into each
+ *                       dense conv's weights and bias (one fold launch per call); every Conv block is one conv launch.
+ *                       images as yb_train_backward, 1 <= batch <= max_batch at the trainer's height x width.  Device
+ *                       outputs, each optional (NULL: not written): pred (B, 4 + nc, A) decoded boxes xywh + class
+ *                       probabilities, boxes (B, 64, A) and scores (B, nc, A) the raw head outputs v8DetectionLoss reads.
+ *                       Asynchronous on `stream`; touches no parameter, running statistic, gradient, Adam moment or
+ *                       BatchNorm ticket counter (it shares the activation arena with the step: one stream at a time). */
 typedef struct yb_trainer yb_trainer;
 int32_t yb_trainer_create(const yb_config* cfg, yb_trainer** out);
 void yb_trainer_destroy(yb_trainer* t);
@@ -283,6 +293,8 @@ int32_t yb_train_step(yb_trainer* t, const void* images, int32_t in_dtype, int32
                       void* stream);
 int32_t yb_get_grad(yb_trainer* t, const char* name, float* out_host, int64_t count);
 int32_t yb_get_tensor(yb_trainer* t, const char* name, float* out_host, int64_t count);
+int32_t yb_trainer_evaluate(yb_trainer* t, const void* images, int32_t in_dtype, int32_t batch, float* pred, float* boxes,
+                            float* scores, void* stream);
 
 /* Replaces (training path of YOLOv11, fp32 parity kernels): the forward and the autograd backward of the depthwise 3x3
  * convolutions - `Convs.DWConv` (Modules/Convs.cs:108-114; groups = gcd(c1, c2) = c for every use in Yolov11: the
@@ -530,6 +542,24 @@ int32_t yb_debug_bneck_f16(const void* x, int32_t batch, int32_t height, int32_t
 int32_t yb_debug_conv_tf32(int32_t pass, const float* x, int32_t x_pitch, const float* dz, const float* w, const float* bias,
                            int32_t n, int32_t height, int32_t width, int32_t cin, int32_t cout, int32_t k, int32_t stride,
                            float* out, void* workspace, int64_t workspace_bytes, char* desc, int32_t desc_capacity);
+/* debug: the eval sibling of yb_debug_conv_tf32 - ONE fold launch and ONE eval-mode conv launch of the Conv block in `eval()`
+ * (Modules/Convs.cs:36-56: SiLU(BatchNorm2d(conv(x))) with the running statistics, eps 1e-3), through the host functions
+ * yb_trainer_evaluate calls; synchronises before it returns.
+ *   out[.., out_coff + c] = [res +] act(conv(x, folded_w) + folded_bias),  act 0 = identity, 1 = SiLU
+ *   x          fp32 NHWC (n, height, width, *), x_pitch 0 = dense (cin), else the element stride between pixels
+ *   w          fp32 (cout, cin, k, k) checkpoint layout; gamma, beta, running_mean, running_var fp32 (cout)
+ *   res        NULL or fp32 NHWC (n, Ho, Wo, *) view added after the activation (the Bottleneck shortcut, Block.cs:606);
+ *              res_pitch 0 = dense (cout)
+ *   out        fp32 NHWC (n, Ho, Wo, out_pitch), written at channels [out_coff, out_coff + cout) only
+ *   folded_w   receives the folded forward operand [k * k][cout][cin]: w * gamma / sqrt(rv + 1e-3), computed in double and
+ *              rounded to fp32 once;  folded_bias receives (cout) beta - rm * gamma / sqrt(rv + 1e-3), likewise
+ *   desc       receives the conv launch's description line (as yb_debug_conv_tf32, kernel name tf_conv_kernel_eval), or NULL
+ * Pitches and out_coff must be multiples of 4 on 16-byte aligned views; k 1 or 3, stride 1 or 2, cin and cout multiples of 8. */
+int32_t yb_debug_conv_tf32_eval(const float* x, int32_t x_pitch, const float* w, const float* gamma, const float* beta,
+                                const float* running_mean, const float* running_var, int32_t n, int32_t height, int32_t width,
+                                int32_t cin, int32_t cout, int32_t k, int32_t stride, int32_t act, const float* res, int32_t res_pitch,
+                                float* out, int32_t out_pitch, int32_t out_coff, float* folded_w, float* folded_bias, char* desc,
+                                int32_t desc_capacity);
 
 #ifdef __cplusplus
 }

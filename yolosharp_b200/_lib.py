@@ -86,6 +86,7 @@ SIGNATURES = {
     "yb_train_step": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_f32, c_f32, c_f32, c_vp, c_vp]),
     "yb_get_grad": (c_i32, [c_vp, c_cp, c_vp, C.c_int64]),
     "yb_get_tensor": (c_i32, [c_vp, c_cp, c_vp, C.c_int64]),
+    "yb_trainer_evaluate": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp]),
     "yb_stem_conv_forward_f32": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp]),
     "yb_stem_conv_backward_weight_f32": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, C.c_int64, c_vp]),
     "yb_dwconv3x3_forward_f32": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp]),
@@ -125,6 +126,8 @@ SIGNATURES = {
                                    c_i32, c_i32, c_vp, c_i32]),
     "yb_debug_conv_tf32": (c_i32, [c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp,
                                    C.c_int64, c_vp, c_i32]),
+    "yb_debug_conv_tf32_eval": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32,
+                                        c_i32, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_i32]),
 }
 
 _lib = None

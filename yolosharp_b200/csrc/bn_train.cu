@@ -28,7 +28,6 @@ static int bn_rows_per_block(long long M) {
   return (int)std::max<long long>(BN_ROWS_PER_BLOCK, (r + BN_TY - 1) / BN_TY * BN_TY);
 }
 
-__device__ __forceinline__ float silu_f(float u) { return u / (1.f + expf(-u)); }
 __device__ __forceinline__ float silu_grad(float u) {
   const float s = 1.f / (1.f + expf(-u));
   return s * (1.f + u * (1.f - s));
@@ -487,18 +486,24 @@ int bn_silu_train_forward(const float* z, long long M, int C, int pitch, const f
     bn_finish_kernel<<<fg, fb, 0, s>>>(3, part, part + (size_t)slabs * C, slabs, C, M, eps, momentum, save_mean, save_invstd, running_mean,
                                        running_var, const_cast<float*>(z) /* the shift row, read only */, nullptr);
   }
+  if (int rc = bn_silu_apply(z, M, C, pitch, save_mean, save_invstd, gamma, beta, act, y, ypitch, s)) return rc;
+  YB_CUDA_CHECK(cudaFreeAsync(part, s));
+  return YB_OK;
+}
+
+int bn_silu_apply(const float* z, long long M, int C, int pitch, const float* mean, const float* invstd, const float* gamma,
+                  const float* beta, int act, float* y, int ypitch, cudaStream_t s) {
   const long long total = M * C;
   if (C % 4 == 0 && pitch % 4 == 0 && ypitch % 4 == 0 && ((uintptr_t)z % 16 == 0) && ((uintptr_t)y % 16 == 0)) {
     const BnRowsPlan pl = bn_rows_plan(M, C);
     BnRows a{};
     a.z = z; a.out = y; a.M = M; a.C = C; a.pitch = pitch; a.opitch = ypitch; a.rpb = pl.rpb; a.act = act;
-    a.mean = save_mean; a.invstd = save_invstd; a.gamma = gamma; a.beta = beta;
+    a.mean = mean; a.invstd = invstd; a.gamma = gamma; a.beta = beta;
     YB_CUDA_CHECK(launch_pdl(bn_rows4_kernel<0>, dim3(pl.colblocks, pl.slabs), dim3(pl.LX, pl.LY), 0, s, a));
   } else {
-    bn_silu_apply_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(z, M, C, pitch, ypitch, save_mean, save_invstd, gamma, beta, act, y);
+    bn_silu_apply_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(z, M, C, pitch, ypitch, mean, invstd, gamma, beta, act, y);
   }
   YB_CUDA_CHECK(cudaGetLastError());
-  YB_CUDA_CHECK(cudaFreeAsync(part, s));
   return YB_OK;
 }
 

@@ -102,6 +102,10 @@ template <> __device__ __forceinline__ float to_f<__half>(__half v) { return __h
 template <typename T> __device__ __forceinline__ T from_f(float v);
 template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
+
+// SiLU, x * sigmoid(x) written as x / (1 + exp(-x)) like ATen's silu kernel: ONE definition for the fp32 CUDA-core
+// kernels, the BatchNorm apply passes of bn_train.cu and the eval epilogue of tf_conv_kernel, so that they round alike
+__device__ __forceinline__ float silu_f(float u) { return u / (1.f + expf(-u)); }
 #endif
 
 // ---- kernels_generic.cu : CUDA-core kernels, templated on storage type (float | __half) ----
@@ -188,6 +192,9 @@ int detection_loss_launch(const float* boxes, const float* scores, int B, int nc
 int bn_silu_train_forward(const float* z, long long M, int C, int pitch, const float* gamma, const float* beta, float eps,
                           float momentum, int act, float* running_mean, float* running_var, float* y, int ypitch,
                           float* save_mean, float* save_invstd, cudaStream_t s, unsigned* counters = nullptr);
+// the elementwise pass alone: y = act(gamma * (z - mean) * invstd + beta) (eval mode: mean / invstd from the running statistics)
+int bn_silu_apply(const float* z, long long M, int C, int pitch, const float* mean, const float* invstd, const float* gamma,
+                  const float* beta, int act, float* y, int ypitch, cudaStream_t s);
 int bn_silu_backward(const float* z, const float* dy, long long M, int C, int pitch, int dpitch, const float* gamma,
                      const float* beta, const float* save_mean, const float* save_invstd, int act, float* dz, int zpitch,
                      float* dgamma, float* dbeta, cudaStream_t s, unsigned* counters = nullptr);
@@ -227,6 +234,21 @@ size_t tf_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, in
 struct TfPackDesc { long long off, chunk0; int cout, cin, taps, pad_; };  // off: element offset in the flat buffers; chunk0: first block
 long long tf_pack_chunks(int cout, int cin, int taps);
 int tf_pack_all(const float* P, float* WF, float* WB, const TfPackDesc* dev_descs, int nd, long long total_chunks, cudaStream_t s);
+// eval mode: BatchNorm (running statistics, eps 1e-3) folded into one conv's forward B operand and bias.  gamma == nullptr:
+// a plain Conv2d, weights packed unscaled; wf == nullptr: per-channel vectors only (bias, invstd: each optional)
+struct TfFoldDesc {
+  const float *w, *gamma, *beta, *rm, *rv;
+  float *wf, *bias, *invstd;
+  long long chunk0;  // first block of this descriptor
+  int cout, cin, taps, pad_;
+};
+long long tf_fold_chunks(const TfFoldDesc& d);
+int tf_fold_all(const TfFoldDesc* dev_descs, int nd, long long total_chunks, cudaStream_t s);
+// eval-mode Conv block on wf (the folded [tap][Cout][Cin] operand): out[.., out_coff + c] = [res +] act(conv(x) + bias), on
+// channel-slice views (pitches in elements, multiples of 4, 16-byte aligned bases)
+int tf_conv_forward_eval(const float* x, int x_pitch, const float* wf, const float* bias, int N, int H, int W, int Cin, int Cout, int k,
+                         int stride, int act, const float* res, int res_pitch, float* out, int out_pitch, int out_coff, cudaStream_t s,
+                         std::string* desc = nullptr);
 int stem3_forward(const float* x, int xc, const float* w, int N, int H, int W, int C, float* z, cudaStream_t s);
 int stem3_backward_weight(const float* x, int xc, const float* dz, int N, int H, int W, int C, float* dw, float* ws, size_t ws_bytes,
                           cudaStream_t s);

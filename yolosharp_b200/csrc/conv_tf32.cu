@@ -52,7 +52,10 @@ struct TfArgs {
   CUtensorMap tmA, tmB;
   TileGrid tg;
   float* out;
-  const float* bias;                // [n_out] or nullptr
+  const float* bias;                // [n_out] or nullptr (always set in the eval epilogue)
+  const float* res;                 // eval epilogue: residual view added after the activation, or nullptr
+  long long r_pitch;                // elements between consecutive output positions of `res`
+  int act;                          // eval epilogue: 1 = SiLU after the bias
   long long o_img, o_row, o_pix;    // element strides of the output addressing
   long long o_off;
   int n_out;                        // valid output channels (columns >= n_out are not stored)
@@ -97,7 +100,10 @@ __device__ __forceinline__ void tf_mainloop(const TfArgs& a, float* acc, uint32_
   wg_fence_acc<NT16 * 8>(acc);
 }
 
-template <int NT16>
+// EVAL = false: out = acc (+ bias), the training forward / dgrad.  EVAL = true: the eval-mode Conv block with BatchNorm
+// folded into the weights and bias, out = [res +] act(acc + bias) (a template parameter, so that the training
+// instantiations carry none of its registers)
+template <int NT16, bool EVAL>
 __global__ void __launch_bounds__(TF_THREADS, NT16 <= 4 ? 2 : 1) tf_conv_kernel(const __grid_constant__ TfArgs a) {
   // the barrier setup below overlaps the tail of the previous kernel (launch_pdl); pdl_wait() before any global access
   extern __shared__ __align__(1024) uint8_t tf_smem[];
@@ -154,12 +160,21 @@ __global__ void __launch_bounds__(TF_THREADS, NT16 <= 4 ? 2 : 1) tf_conv_kernel(
         const int ho = tc.th * a.BH + hl, wo = tc.tw * a.BW + wl;
         if (hl >= a.BH || ho >= a.Ho || wo >= a.Wo) continue;
         float* orow = a.out + (long long)tc.img * a.o_img + (long long)ho * a.o_row + (long long)wo * a.o_pix + a.o_off + n0;
+        const float* rrow = EVAL && a.res ? a.res + (((long long)tc.img * a.Ho + ho) * a.Wo + wo) * a.r_pitch + n0 : nullptr;
 #pragma unroll
         for (int J = 0; J < NT16 * 2; J++) {
           const int c = 8 * J + 2 * t4;
           if (n0 + c < a.n_out) {  // n_out is a multiple of 4
             float2 o = make_float2(acc[4 * J + 2 * h], acc[4 * J + 2 * h + 1]);
-            if (a.bias) {
+            if (EVAL) {
+              const float2 b = *reinterpret_cast<const float2*>(a.bias + n0 + c);
+              o.x += b.x; o.y += b.y;
+              if (a.act) { o.x = silu_f(o.x); o.y = silu_f(o.y); }
+              if (rrow) {  // the Bottleneck shortcut, `x + cv2(cv1(x))` (Block.cs:606)
+                const float2 r = *reinterpret_cast<const float2*>(rrow + c);
+                o.x = r.x + o.x; o.y = r.y + o.y;
+              }
+            } else if (a.bias) {
               const float2 b = *reinterpret_cast<const float2*>(a.bias + n0 + c);
               o.x += b.x; o.y += b.y;
             }
@@ -213,6 +228,55 @@ __global__ void __launch_bounds__(256) tf_pack_all_kernel(const float* __restric
   }
 }
 long long tf_pack_chunks(int cout, int cin, int taps) { return ((long long)cout * cin * taps + TF_PACK_CHUNK - 1) / TF_PACK_CHUNK; }
+
+// Eval-mode BatchNorm folded into every conv of a model in ONE launch (Conv block in `eval()`, Convs.cs:36-56):
+//   wf[tap][co][ci] = w[co][ci][tap] * s[co],  bias[co] = beta[co] - rm[co] * s[co],  s = gamma / sqrt(rv + 1e-3)
+// computed in double and rounded to fp32 once, as the engine folds on the host (DESIGN.md §3); explicit _rn intrinsics keep
+// the compiler from contracting them into FMAs, so the result is the float64 fold rounded to fp32 bit for bit.  invstd[co] =
+// 1 / sqrt(rv + 1e-3) serves the convs without a bias epilogue (stem, depthwise), which apply BatchNorm as a separate pass.
+// A descriptor without gamma (a plain Conv2d) packs its weights unscaled.  Block b works on chunk b - chunk0 of the
+// descriptor that owns it; chunk 0 of each descriptor also writes the per-channel vectors.
+__global__ void __launch_bounds__(256) tf_fold_all_kernel(const TfFoldDesc* __restrict__ d, int nd) {
+  int lo = 0, hi = nd - 1;  // last descriptor whose first chunk <= blockIdx.x
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (d[mid].chunk0 <= (long long)blockIdx.x) lo = mid; else hi = mid - 1;
+  }
+  const TfFoldDesc L = d[lo];
+  const long long c0 = (long long)blockIdx.x - L.chunk0;
+  auto scale = [&](int co) {
+    return L.gamma ? __ddiv_rn((double)L.gamma[co], __dsqrt_rn(__dadd_rn((double)L.rv[co], 1e-3))) : 1.0;
+  };
+  if (c0 == 0 && L.gamma)
+    for (int co = threadIdx.x; co < L.cout; co += 256) {
+      const double s = scale(co);
+      if (L.bias) L.bias[co] = (float)__dsub_rn((double)L.beta[co], __dmul_rn((double)L.rm[co], s));
+      if (L.invstd) L.invstd[co] = (float)__ddiv_rn(1.0, __dsqrt_rn(__dadd_rn((double)L.rv[co], 1e-3)));
+    }
+  if (!L.wf) return;
+  const long long n = (long long)L.cout * L.cin * L.taps;
+  const long long i0 = c0 * TF_PACK_CHUNK, i1 = min(n, i0 + TF_PACK_CHUNK);
+  // the scales of the output channels this chunk touches (at most one per element), once per channel
+  __shared__ double sc[TF_PACK_CHUNK];
+  const long long per_co = (long long)L.cin * L.taps;
+  const int co0 = (int)(i0 / per_co), nco = (int)((i1 - 1) / per_co) - co0 + 1;
+  if (L.gamma)
+    for (int j = threadIdx.x; j < nco; j += 256) sc[j] = scale(co0 + j);
+  __syncthreads();
+  for (long long i = i0 + threadIdx.x; i < i1; i += 256) {
+    const int t = (int)(i % L.taps);
+    const long long q = i / L.taps;
+    const int ci = (int)(q % L.cin), co = (int)(q / L.cin);
+    L.wf[((size_t)t * L.cout + co) * L.cin + ci] = L.gamma ? (float)__dmul_rn((double)L.w[i], sc[co - co0]) : L.w[i];
+  }
+}
+long long tf_fold_chunks(const TfFoldDesc& d) { return d.wf ? std::max(1ll, tf_pack_chunks(d.cout, d.cin, d.taps)) : 1; }
+int tf_fold_all(const TfFoldDesc* dev_descs, int nd, long long total_chunks, cudaStream_t s) {
+  if (nd <= 0 || total_chunks <= 0) return YB_OK;
+  tf_fold_all_kernel<<<(unsigned)total_chunks, 256, 0, s>>>(dev_descs, nd);
+  YB_CUDA_CHECK(cudaGetLastError());
+  return YB_OK;
+}
 int tf_pack_all(const float* P, float* WF, float* WB, const TfPackDesc* dev_descs, int nd, long long total_chunks, cudaStream_t s) {
   if (nd <= 0 || total_chunks <= 0) return YB_OK;
   tf_pack_all_kernel<<<(unsigned)total_chunks, 256, 0, s>>>(P, WF, WB, dev_descs, nd);
@@ -227,6 +291,8 @@ struct TfLaunch {
   const float* wpk; int Nc, taps_total;
   float* out; long long o_img, o_row, o_pix, o_off;
   const float* bias;
+  bool eval;         // eval epilogue: out = [res +] act(acc + bias)
+  const float* res; long long r_pitch; int act;
   int Ho, Wo;        // output position grid
   int in_stride;
   int ntaps; int dh[9], dw[9], slab[9];
@@ -240,6 +306,7 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
   TfArgs a;
   memset(&a, 0, sizeof(a));
   a.out = L.out; a.bias = L.bias;
+  a.res = L.res; a.r_pitch = L.r_pitch; a.act = L.act;
   a.o_img = L.o_img; a.o_row = L.o_row; a.o_pix = L.o_pix; a.o_off = L.o_off;
   a.n_out = L.Nc;
   a.in_stride = L.in_stride;
@@ -305,14 +372,16 @@ static int tf_conv_launch(const TfLaunch& L, cudaStream_t s, std::string* desc) 
   if (a.stages < 2) { set_error("tf32 conv: tile does not fit in shared memory"); return YB_ERR_SHAPE; }
   const size_t smem = (size_t)a.stages * (a.a_stride + a.b_stride) + 1024;
   void (*kernel)(TfArgs) = nullptr;
-  dispatch_nt16(a.n_tile / 16, [&](auto nt16) { kernel = tf_conv_kernel<decltype(nt16)::value>; });
+  dispatch_nt16(a.n_tile / 16, [&](auto nt16) {
+    kernel = L.eval ? tf_conv_kernel<decltype(nt16)::value, true> : tf_conv_kernel<decltype(nt16)::value, false>;
+  });
   YB_CUDA_CHECK(smem_limit((const void*)kernel, smem, false));
   const int grid = std::min(a.tg.total, occ * sm_count());
   if (desc) {
     char line[256];
-    snprintf(line, sizeof(line), "%stf_conv_kernel BK %d chunks %d n_tile %d x%d BW %d BH %d in_stride %d flat %d ntaps %d occ %d stages %d grid %d",
-             desc->empty() ? "" : "\n", a.BK, a.chunks, a.n_tile, a.tg.n_tiles, a.BW, a.BH, a.in_stride, L.flat ? 1 : 0, a.ntaps, occ,
-             a.stages, grid);
+    snprintf(line, sizeof(line), "%stf_conv_kernel%s BK %d chunks %d n_tile %d x%d BW %d BH %d in_stride %d flat %d ntaps %d occ %d stages %d grid %d",
+             desc->empty() ? "" : "\n", L.eval ? "_eval" : "", a.BK, a.chunks, a.n_tile, a.tg.n_tiles, a.BW, a.BH, a.in_stride, L.flat ? 1 : 0,
+             a.ntaps, occ, a.stages, grid);
     *desc += line;
   }
   YB_CUDA_CHECK(launch_pdl(kernel, dim3(grid), dim3(TF_THREADS), smem, s, a));
@@ -344,6 +413,31 @@ int tf_conv_forward(const float* x, const float* w, const float* bias, int N, in
   L.ntaps = k * k;
   for (int t = 0; t < k * k; t++) { L.dh[t] = t / k - pad; L.dw[t] = t % k - pad; L.slab[t] = t; }
   L.flat = (k == 1 && stride == 1);
+  return tf_conv_launch(L, s, desc);
+}
+
+int tf_conv_forward_eval(const float* x, int x_pitch, const float* wf, const float* bias, int N, int H, int W, int Cin, int Cout, int k,
+                         int stride, int act, const float* res, int res_pitch, float* out, int out_pitch, int out_coff, cudaStream_t s,
+                         std::string* desc) {
+  auto view_ok = [](const void* p, int pitch, int C) { return pitch >= C && pitch % 4 == 0 && ((uintptr_t)p & 15) == 0; };
+  if (!view_ok(x, x_pitch, Cin) || !view_ok(out, out_pitch, out_coff + Cout) || out_coff < 0 || out_coff % 4 || (res && !view_ok(res, res_pitch, Cout))) {
+    set_error("tf32 eval conv: input / output / residual views must be 16-byte aligned with pitches and channel offset multiples of 4");
+    return YB_ERR_SHAPE;
+  }
+  if (!tf_shape_ok(Cin, Cout, k, stride, k / 2)) { set_error("tf32 eval conv: channels must be multiples of 8, k in {1,3}, stride in {1,2}"); return YB_ERR_SHAPE; }
+  const int pad = k / 2;
+  TfLaunch L;
+  memset(&L, 0, sizeof(L));
+  L.in = x; L.N = N; L.Hi = H; L.Wi = W; L.Kc = Cin; L.in_pitch = x_pitch;
+  L.wpk = wf; L.Nc = Cout; L.taps_total = k * k;
+  L.Ho = (H + 2 * pad - k) / stride + 1; L.Wo = (W + 2 * pad - k) / stride + 1;
+  L.out = out; L.o_pix = out_pitch; L.o_row = (long long)L.Wo * out_pitch; L.o_img = (long long)L.Ho * L.o_row; L.o_off = out_coff;
+  L.bias = bias;
+  L.eval = true; L.res = res; L.r_pitch = res_pitch; L.act = act;
+  L.in_stride = stride;
+  L.ntaps = k * k;
+  for (int t = 0; t < k * k; t++) { L.dh[t] = t / k - pad; L.dw[t] = t % k - pad; L.slab[t] = t; }
+  L.flat = (k == 1 && stride == 1);  // positions are addressed through the pitches, so views flatten like dense tensors
   return tf_conv_launch(L, s, desc);
 }
 
@@ -945,6 +1039,47 @@ int32_t yb_debug_conv_tf32(int32_t pass, const float* x, int32_t x_pitch, const 
     set_error(std::string("yb_debug_conv_tf32: kernel failed: ") + cudaGetErrorString(ce));
     rc = YB_ERR_CUDA;
   }
+  if (desc && desc_capacity > 0) snprintf(desc, (size_t)desc_capacity, "%s", d.c_str());
+  return rc;
+}
+
+int32_t yb_debug_conv_tf32_eval(const float* x, int32_t x_pitch, const float* w, const float* gamma, const float* beta,
+                                const float* running_mean, const float* running_var, int32_t n, int32_t height, int32_t width,
+                                int32_t cin, int32_t cout, int32_t k, int32_t stride, int32_t act, const float* res, int32_t res_pitch,
+                                float* out, int32_t out_pitch, int32_t out_coff, float* folded_w, float* folded_bias, char* desc,
+                                int32_t desc_capacity) {
+  if (!x || !w || !gamma || !beta || !running_mean || !running_var || !out || !folded_w || !folded_bias) {
+    set_error("yb_debug_conv_tf32_eval: null argument");
+    return YB_ERR_INVALID_ARG;
+  }
+  if (n <= 0 || height <= 0 || width <= 0 || cin <= 0 || cout <= 0 || x_pitch < 0 || res_pitch < 0 || out_pitch <= 0 || (act != 0 && act != 1)) {
+    set_error("yb_debug_conv_tf32_eval: bad argument (extent, pitch or act)");
+    return YB_ERR_INVALID_ARG;
+  }
+  if (!tf_shape_ok(cin, cout, k, stride, k / 2)) {
+    set_error("yb_debug_conv_tf32_eval: shape not supported: channels must be multiples of 8, k in {1,3}, stride in {1,2}");
+    return YB_ERR_SHAPE;
+  }
+  if (!have_device("yb_debug_conv_tf32_eval")) return YB_ERR_NO_DEVICE;
+  TfFoldDesc fd{};
+  fd.w = w; fd.gamma = gamma; fd.beta = beta; fd.rm = running_mean; fd.rv = running_var;
+  fd.wf = folded_w; fd.bias = folded_bias;
+  fd.cout = cout; fd.cin = cin; fd.taps = k * k;
+  TfFoldDesc* dd = nullptr;
+  YB_CUDA_CHECK(cudaMalloc((void**)&dd, sizeof(TfFoldDesc)));
+  std::string d;
+  int rc = cudaMemcpy(dd, &fd, sizeof(fd), cudaMemcpyHostToDevice) == cudaSuccess ? 0 : YB_ERR_CUDA;
+  if (rc) set_error("yb_debug_conv_tf32_eval: descriptor copy failed");
+  if (!rc) rc = tf_fold_all(dd, 1, tf_fold_chunks(fd), 0);
+  if (!rc)
+    rc = tf_conv_forward_eval(x, x_pitch ? x_pitch : cin, folded_w, folded_bias, n, height, width, cin, cout, k, stride, act, res,
+                              res_pitch ? res_pitch : cout, out, out_pitch, out_coff, 0, &d);
+  const cudaError_t ce = cudaDeviceSynchronize();
+  if (!rc && ce != cudaSuccess) {
+    set_error(std::string("yb_debug_conv_tf32_eval: kernel failed: ") + cudaGetErrorString(ce));
+    rc = YB_ERR_CUDA;
+  }
+  cudaFree(dd);
   if (desc && desc_capacity > 0) snprintf(desc, (size_t)desc_capacity, "%s", d.c_str());
   return rc;
 }

@@ -10,11 +10,6 @@
 
 namespace yb {
 
-__device__ __forceinline__ float silu_f(float x) {
-  // x * sigmoid(x), written as x / (1 + exp(-x)) like ATen's silu kernel
-  return x / (1.0f + expf(-x));
-}
-
 // ------------------------------------------------------------------------------------------
 // Generic implicit-GEMM convolution on CUDA cores.
 //   M = B*Ho*Wo output pixels, N = Cout, K = k*k*Cin (tap-major).  64x64 tile, 16-deep slabs,

@@ -278,6 +278,15 @@ struct Net {
   long long pack_chunks = 0;
   int step_count = 0;
   int rc = 0;  // first error of the current step (modules return empty tensors after it)
+  // eval mode (yb_trainer_evaluate): BatchNorm on the running statistics, folded by ONE launch per forward into EV, a
+  // parameter-sized buffer laid out like P: a dense conv's folded [tap][Cout][Cin] operand at its weight's offset, the folded
+  // bias at its bn.bias offset, 1 / sqrt(rv + eps) at its bn.weight offset (read by the stem and depthwise convs, whose
+  // BatchNorm stays a separate pass); the head's plain Conv2d weights packed unscaled at their offset
+  bool eval = false;
+  float* EV = nullptr;
+  TfFoldDesc* fold_descs = nullptr;
+  int n_folds = 0;
+  long long fold_chunks = 0;
 
   float* alloc(long long n) {
     const size_t bytes = ((size_t)n * sizeof(float) + 255) & ~(size_t)255;
@@ -296,6 +305,7 @@ struct Net {
   const float* wb(const std::string& k) { return WB ? WB + params[pidx.at(k)].off : nullptr; }
   float* g(const std::string& k) { return G + params[pidx.at(k)].off; }
   float* r(const std::string& k) { return R + stats[sidx.at(k)].off; }
+  float* ev(const std::string& k) { return EV + params[pidx.at(k)].off; }
   void check(int code) { if (code && !rc) rc = code; }
   void check_launch() { if (!rc && cudaGetLastError() != cudaSuccess) { rc = YB_ERR_CUDA; set_error("yb_train_step: kernel launch failed"); } }
 };
@@ -358,6 +368,7 @@ struct Conv : Module {
     (void)n;
   }
   T4 forward(Net& n, T4 in, const T4* dst = nullptr) override {
+    if (n.eval) return forward_eval(n, in, dst, nullptr);
     x = depthwise ? dense_copy(n, in) : in;  // the depthwise kernels take dense tensors
     const int Ho = (in.H + 2 * (k / 2) - k) / s + 1, Wo = (in.W + 2 * (k / 2) - k) / s + 1;
     z = n.make(in.N, Ho, Wo, cout);
@@ -381,6 +392,29 @@ struct Conv : Module {
     }
     n.check(bn_silu_train_forward(z.p, z.rows(), cout, cout, n.p(name + ".bn.weight"), n.p(name + ".bn.bias"), 1e-3f, 0.03f, act,
                                   n.r(name + ".bn.running_mean"), n.r(name + ".bn.running_var"), y.p, y.pitch, mean, invstd, n.s, n.bn_counters));
+    return y;
+  }
+  // eval mode (Convs.cs:36-56 in `eval()`): a dense conv is ONE launch on the folded operands, + res after the activation
+  // when given; the stem and depthwise convs keep their forward kernel and apply BatchNorm with the running statistics
+  T4 forward_eval(Net& n, T4 in, const T4* dst, const T4* res) {
+    const int Ho = (in.H + 2 * (k / 2) - k) / s + 1, Wo = (in.W + 2 * (k / 2) - k) / s + 1;
+    T4 y = dst ? *dst : n.make(in.N, Ho, Wo, cout);
+    if (n.rc) return y;
+    const bool stem = pad8 && k == 3 && s == 2 && cout % 8 == 0 && cout <= 128;
+    if (!depthwise && !stem) {
+      if (pad8) { n.check(YB_ERR_SHAPE); set_error("yb_trainer_evaluate: the stem needs cout % 8 == 0 and cout <= 128"); return y; }
+      n.check(tf_conv_forward_eval(in.p, in.pitch, n.ev(name + ".conv.weight"), n.ev(name + ".bn.bias"), in.N, in.H, in.W, cin, cout, k, s,
+                                   act, res ? res->p : nullptr, res ? res->pitch : 0, y.p, y.pitch, 0, n.s));
+      return y;
+    }
+    const T4 xin = depthwise ? dense_copy(n, in) : in;
+    T4 zz = n.make(in.N, Ho, Wo, cout);
+    if (n.rc) return y;
+    const float* w = n.p(name + ".conv.weight");
+    if (depthwise) n.check(dwconv3x3_forward_f32(xin.p, w, xin.N, xin.H, xin.W, xin.C, zz.p, n.s));
+    else n.check(stem3_forward(xin.p, 8, w, xin.N, xin.H, xin.W, cout, zz.p, n.s));
+    n.check(bn_silu_apply(zz.p, zz.rows(), cout, cout, n.r(name + ".bn.running_mean"), n.ev(name + ".bn.weight"), n.p(name + ".bn.weight"),
+                          n.p(name + ".bn.bias"), act, y.p, y.pitch, n.s));
     return y;
   }
   T4 backward(Net& n, T4 dy) override {
@@ -426,6 +460,11 @@ struct Conv2dBias : Module {
     x = in;
     T4 y = n.make(in.N, in.H, in.W, cout);
     if (n.rc) return y;
+    if (n.eval) {  // the packed weights of the step (WF) may predate the last optimizer step: EV holds the current ones
+      n.check(tf_conv_forward_eval(in.p, in.pitch, n.ev(name + ".weight"), n.p(name + ".bias"), in.N, in.H, in.W, cin, cout, 1, 1, 0, nullptr, 0,
+                                   y.p, y.pitch, 0, n.s));
+      return y;
+    }
     n.check(tf_conv_forward(in.p, n.p(name + ".weight"), n.p(name + ".bias"), in.N, in.H, in.W, cin, cout, 1, 1, 0, y.p, n.ws, n.ws_bytes, n.s,
                             in.dense() ? 0 : in.pitch, n.wf(name + ".weight")));
     return y;
@@ -466,6 +505,7 @@ struct Bottleneck : Module {
       : cv1(n, nm + ".cv1", c1, (int)(c2 * e), 3), cv2(n, nm + ".cv2", (int)(c2 * e), c2, 3), add_(shortcut && c1 == c2) {}
   T4 forward(Net& n, T4 x, const T4* dst = nullptr) override {
     if (!add_) return cv2.forward(n, cv1.forward(n, x), dst);
+    if (n.eval) return cv2.forward_eval(n, cv1.forward(n, x), dst, &x);  // the shortcut add in cv2's epilogue
     T4 y = cv2.forward(n, cv1.forward(n, x));
     T4 out = dst ? *dst : n.make(x.N, x.H, x.W, x.C);
     add_into(n, out, x, y);
@@ -688,7 +728,9 @@ struct Detect {
       cv3[i].layers.emplace_back(new Conv2dBias(c + ".2", c3, nc));
     }
   }
-  void forward(Net& n, const T4 feats[3], float* boxes, float* scores, int A) {
+  // boxes / scores: the raw outputs (B, C, A), each skipped when null (eval); pred: the decoded (B, 4 + nc, A) of the fp32
+  // engine (`Detect._inference`, Head.cs:204-223), written when given
+  void forward(Net& n, const T4 feats[3], float* boxes, float* scores, int A, float* pred = nullptr) {
     shapes.assign(feats, feats + 3);
     int a0 = 0;
     for (int i = 0; i < 3; i++) {
@@ -696,9 +738,15 @@ struct Detect {
       T4 s = cv3[i].forward(n, feats[i]);
       if (n.rc) return;
       const int hw = feats[i].H * feats[i].W;
-      nhwc_to_bca_kernel<<<nb((long long)b.N * hw * b.C), 256, 0, n.s>>>(b.p, boxes, b.N, hw, b.C, A, a0);
-      nhwc_to_bca_kernel<<<nb((long long)s.N * hw * s.C), 256, 0, n.s>>>(s.p, scores, s.N, hw, s.C, A, a0);
+      if (boxes) nhwc_to_bca_kernel<<<nb((long long)b.N * hw * b.C), 256, 0, n.s>>>(b.p, boxes, b.N, hw, b.C, A, a0);
+      if (scores) nhwc_to_bca_kernel<<<nb((long long)s.N * hw * s.C), 256, 0, n.s>>>(s.p, scores, s.N, hw, s.C, A, a0);
       n.check_launch();
+      if (pred) {
+        View vb, vc;
+        vb.base = b.p; vb.H = b.H; vb.W = b.W; vb.pitch = b.pitch; vb.C = b.C;
+        vc.base = s.p; vc.H = s.H; vc.W = s.W; vc.pitch = s.pitch; vc.C = s.C;
+        n.check(launch_decode_level<float>(vb, vc, nullptr, b.N, nc, 0, reg_max, (float)(n.H / b.H), a0, A, 4 + nc, pred, n.s));
+      }
       a0 += hw;
     }
   }
@@ -931,6 +979,42 @@ size_t max_workspace(yb_trainer* t) {
   return sw.ws + 4096;
 }
 
+// the layer walk of Yolo.cs:92-134 up to the Detect head, in train or eval mode (n.eval): saves the outputs the concats and
+// the backward pass read, returns the three head inputs
+int forward_layers(yb_trainer* t, T4 x, T4 feats[3]) {
+  Net& n = t->net;
+  t->outputs.clear();
+  t->cat_split.clear();
+  t->up_in.clear();
+  int cat_count = 0;
+  for (size_t i = 0; i < t->layers.size() && !n.rc; i++) {
+    Layer& l = t->layers[i];
+    if (l.kind == 1) {
+      T4 y = n.make(x.N, 2 * x.H, 2 * x.W, x.C);
+      if (n.rc) break;
+      up2_forward_kernel<<<nb(y.numel()), 256, 0, n.s>>>(x.p, x.pitch, y.p, y.pitch, x.N, x.H, x.W, x.C);
+      n.check_launch();
+      t->up_in.push_back(x);
+      x = y;
+    } else if (l.kind == 2) {
+      const T4& other = t->outputs[t->concat_index[cat_count]];
+      t->cat_split.push_back({x.C, t->concat_index[cat_count]});
+      T4 y = n.make(x.N, x.H, x.W, x.C + other.C);
+      put(n, y, 0, x);
+      put(n, y, x.C, other);
+      x = y;
+      cat_count++;
+    } else {
+      x = l.m->forward(n, x);
+    }
+    if (std::find(t->output_idx.begin(), t->output_idx.end(), (int)i) != t->output_idx.end()) t->outputs.push_back(x);
+  }
+  if (n.rc) return n.rc;
+  const int n_out = (int)t->outputs.size();
+  for (int k = 0; k < 3; k++) feats[k] = t->outputs[n_out - 3 + k];
+  return YB_OK;
+}
+
 // forward + loss + backward of one batch; gradients land in the caller's flat buffer
 int run_backward(yb_trainer* t, const void* images, int in_dtype, int B, const float* targets_host, int n_targets, float* items_host,
                  cudaStream_t s) {
@@ -962,36 +1046,9 @@ int run_backward(yb_trainer* t, const void* images, int in_dtype, int B, const f
   images_to_nhwc8_kernel<<<nb((long long)B * H * W), 256, 0, s>>>(images, in_dtype == YB_U8 ? 1 : 0, x.p, B, H, W);
   n.check_launch();
   n.check(tf_pack_all(n.P, n.WF, n.WB, n.pack_descs, n.n_packs, n.pack_chunks, s));  // the weights as this step sees them
-  // ---- forward (Yolo.cs:92-134) ----
-  t->outputs.clear();
-  t->cat_split.clear();
-  t->up_in.clear();
-  int cat_count = 0;
-  for (size_t i = 0; i < t->layers.size() && !n.rc; i++) {
-    Layer& l = t->layers[i];
-    if (l.kind == 1) {
-      T4 y = n.make(x.N, 2 * x.H, 2 * x.W, x.C);
-      if (n.rc) break;
-      up2_forward_kernel<<<nb(y.numel()), 256, 0, s>>>(x.p, x.pitch, y.p, y.pitch, x.N, x.H, x.W, x.C);
-      n.check_launch();
-      t->up_in.push_back(x);
-      x = y;
-    } else if (l.kind == 2) {
-      const T4& other = t->outputs[t->concat_index[cat_count]];
-      t->cat_split.push_back({x.C, t->concat_index[cat_count]});
-      T4 y = n.make(x.N, x.H, x.W, x.C + other.C);
-      put(n, y, 0, x);
-      put(n, y, x.C, other);
-      x = y;
-      cat_count++;
-    } else {
-      x = l.m->forward(n, x);
-    }
-    if (std::find(t->output_idx.begin(), t->output_idx.end(), (int)i) != t->output_idx.end()) t->outputs.push_back(x);
-  }
-  if (n.rc) return n.rc;
+  T4 feats[3];
+  if (int rc = forward_layers(t, x, feats)) return rc;
   const int n_out = (int)t->outputs.size();
-  const T4 feats[3] = {t->outputs[n_out - 3], t->outputs[n_out - 2], t->outputs[n_out - 1]};
   const int A = feats[0].H * feats[0].W + feats[1].H * feats[1].W + feats[2].H * feats[2].W;
   t->A = A;
   t->boxes = n.alloc((long long)B * 64 * A);
@@ -1058,6 +1115,51 @@ int run_backward(yb_trainer* t, const void* images, int in_dtype, int B, const f
     }
   }
   t->last_batch = B;
+  return YB_OK;
+}
+
+// eval mode: the fold descriptors of every conv (pointers into the bound buffers and EV), built on first use after a bind
+int prepare_eval(yb_trainer* t) {
+  Net& n = t->net;
+  if (n.fold_descs) return YB_OK;
+  if (!n.EV && cudaMalloc((void**)&n.EV, (size_t)n.n_params * sizeof(float)) != cudaSuccess) {
+    n.EV = nullptr;
+    cudaGetLastError();
+    set_error("yb_trainer_evaluate: cudaMalloc of the folded weight buffer failed");
+    return YB_ERR_CUDA;
+  }
+  std::vector<TfFoldDesc> d;
+  long long chunk = 0;
+  const std::string cw = ".conv.weight";
+  for (auto& e : n.params) {
+    if (e.shape.size() != 4) continue;
+    TfFoldDesc q{};
+    q.w = n.P + e.off;
+    q.cout = (int)e.shape[0]; q.cin = (int)e.shape[1]; q.taps = (int)(e.shape[2] * e.shape[3]);
+    const bool dense = q.cout % 8 == 0 && q.cin % 8 == 0;  // the stem (3 channels) and depthwise convs keep their own kernels
+    if (e.name.size() > cw.size() && e.name.compare(e.name.size() - cw.size(), cw.size(), cw) == 0) {
+      const std::string b = e.name.substr(0, e.name.size() - cw.size());
+      q.gamma = n.p(b + ".bn.weight"); q.beta = n.p(b + ".bn.bias");
+      q.rm = n.r(b + ".bn.running_mean"); q.rv = n.r(b + ".bn.running_var");
+      q.bias = n.ev(b + ".bn.bias"); q.invstd = n.ev(b + ".bn.weight");
+    } else if (!dense) {
+      continue;  // a plain Conv2d the eval forward does not run on the tensor cores (none in the detect graphs)
+    }
+    q.wf = dense ? n.EV + e.off : nullptr;
+    q.chunk0 = chunk;
+    chunk += tf_fold_chunks(q);
+    d.push_back(q);
+  }
+  if (cudaMalloc((void**)&n.fold_descs, std::max<size_t>(1, d.size()) * sizeof(TfFoldDesc)) != cudaSuccess ||
+      cudaMemcpy(n.fold_descs, d.data(), d.size() * sizeof(TfFoldDesc), cudaMemcpyHostToDevice) != cudaSuccess) {
+    if (n.fold_descs) cudaFree(n.fold_descs);
+    n.fold_descs = nullptr;
+    cudaGetLastError();
+    set_error("yb_trainer_evaluate: fold descriptor upload failed");
+    return YB_ERR_CUDA;
+  }
+  n.n_folds = (int)d.size();
+  n.fold_chunks = chunk;
   return YB_OK;
 }
 
@@ -1142,6 +1244,8 @@ void yb_trainer_destroy(yb_trainer* t) {
   if (t->net.WB) cudaFree(t->net.WB);
   if (t->net.pack_descs) cudaFree(t->net.pack_descs);
   if (t->net.bn_counters) cudaFree(t->net.bn_counters);
+  if (t->net.EV) cudaFree(t->net.EV);
+  if (t->net.fold_descs) cudaFree(t->net.fold_descs);
   if (t->tg_pinned) cudaFreeHost(t->tg_pinned);
   if (t->tg_copied) cudaEventDestroy(t->tg_copied);
   delete t;
@@ -1174,6 +1278,7 @@ int64_t yb_trainer_flat_size(const yb_trainer* t, int32_t kind) {
 int32_t yb_trainer_bind(yb_trainer* t, float* params, float* grads, float* adam_m, float* adam_v, float* running_stats) {
   if (!t || !params || !grads || !adam_m || !adam_v || !running_stats) { set_error("yb_trainer_bind: null argument"); return YB_ERR_INVALID_ARG; }
   t->net.P = params; t->net.G = grads; t->net.M1 = adam_m; t->net.M2 = adam_v; t->net.R = running_stats;
+  if (t->net.fold_descs) { cudaFree(t->net.fold_descs); t->net.fold_descs = nullptr; }  // they point into the old buffers
   return YB_OK;
 }
 
@@ -1206,6 +1311,37 @@ int32_t yb_train_step(yb_trainer* t, const void* images, int32_t in_dtype, int32
                       float lr_bias, float lr_other, float weight_decay, float* loss_items_host, void* stream) {
   if (int rc = yb_train_backward(t, images, in_dtype, batch, targets_host, n_targets, loss_items_host, stream)) return rc;
   return yb_train_apply(t, lr_bias, lr_other, weight_decay, stream);
+}
+
+int32_t yb_trainer_evaluate(yb_trainer* t, const void* images, int32_t in_dtype, int32_t batch, float* pred, float* boxes,
+                            float* scores, void* stream) {
+  if (!t || !images) { set_error("yb_trainer_evaluate: null argument"); return YB_ERR_INVALID_ARG; }
+  if (!t->net.P || !t->net.arena) { set_error("yb_trainer_evaluate: call yb_trainer_bind first (and create without DRY_RUN)"); return YB_ERR_STATE; }
+  if (batch <= 0 || batch > t->net.max_batch) { set_error("yb_trainer_evaluate: batch outside [1, max_batch]"); return YB_ERR_INVALID_ARG; }
+  if (in_dtype != YB_U8 && in_dtype != YB_F32) { set_error("yb_trainer_evaluate: images must be u8 or f32 NCHW"); return YB_ERR_INVALID_ARG; }
+  if (!have_device("yb_trainer_evaluate")) return YB_ERR_NO_DEVICE;
+  if (int rc = prepare_eval(t)) return rc;
+  Net& n = t->net;
+  cudaStream_t s = (cudaStream_t)stream;
+  n.s = s;
+  n.rc = 0;
+  n.arena_off = 0;
+  const int H = n.H, W = n.W;
+  T4 x = n.make(batch, H, W, 8);
+  if (n.rc) return n.rc;
+  images_to_nhwc8_kernel<<<nb((long long)batch * H * W), 256, 0, s>>>(images, in_dtype == YB_U8 ? 1 : 0, x.p, batch, H, W);
+  n.check_launch();
+  n.check(tf_fold_all(n.fold_descs, n.n_folds, n.fold_chunks, s));  // BatchNorm as the current parameters and statistics give it
+  n.eval = true;
+  T4 feats[3];
+  int rc = forward_layers(t, x, feats);
+  if (!rc) {
+    const int A = feats[0].H * feats[0].W + feats[1].H * feats[1].W + feats[2].H * feats[2].W;
+    t->detect->forward(n, feats, boxes, scores, A, pred);
+    rc = n.rc;
+  }
+  n.eval = false;
+  return rc;
 }
 
 int32_t yb_get_grad(yb_trainer* t, const char* name, float* out_host, int64_t count) {

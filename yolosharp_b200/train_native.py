@@ -38,6 +38,7 @@ class NativeTrainer:
         self._h = C.c_void_p()
         L.check(L.lib().yb_trainer_create(C.byref(cfg), C.byref(self._h)))
         self.nc, self.step_count, self.group = nc, 0, None
+        self.max_batch, self.height, self.width = max_batch, height, width
         self.lr = lr if lr is not None else round(0.002 * 5 / (4 + nc), 6)  # YoloBaseTaskModel.cs:142
         self.wd = weight_decay
         self.params, self.stats = self._layout(0), self._layout(1)
@@ -106,6 +107,31 @@ class NativeTrainer:
         L.check(L.lib().yb_train_apply(self._h, lr_bias, lr_other, self.wd, sp))
         self.step_count += 1
         return items
+
+    def evaluate(self, images_nchw, stream=None):
+        """`AMPWrapper.Evaluate` (Utils/Amp.cs:387-395): the model being trained in `eval()` - BatchNorm on the running
+        statistics, TF32 tensor-core convolutions, fp32 storage - on images (B,3,H,W) uint8 or float32 in [0,1] on the device,
+        B <= max_batch at the trainer's H x W.  Changes no parameter, running statistic, gradient or Adam moment.
+        -> (pred (B, 4+nc, A) decoded xywh + class probabilities, boxes (B, 64, A), scores (B, nc, A) raw head outputs),
+        device tensors written on `stream` (default: the current stream)."""
+        if not (torch.is_tensor(images_nchw) and images_nchw.dim() == 4 and images_nchw.shape[1] == 3 and
+                images_nchw.dtype in (torch.uint8, torch.float32)):
+            raise ValueError("evaluate: images must be a (B, 3, H, W) uint8 or float32 tensor")
+        B, _, H, W = images_nchw.shape
+        if B < 1 or B > self.max_batch or (H, W) != (self.height, self.width):
+            raise ValueError(f"evaluate: batch {B} x {H} x {W}, the trainer takes 1..{self.max_batch} x {self.height} x {self.width}")
+        if self.device.type != "cuda":
+            raise RuntimeError("evaluate: this trainer was created without a device (layout only)")
+        assert images_nchw.is_cuda and images_nchw.is_contiguous()
+        A = sum((H // s) * (W // s) for s in (8, 16, 32))
+        pred = torch.empty(B, 4 + self.nc, A, dtype=torch.float32, device=self.device)
+        boxes = torch.empty(B, 64, A, dtype=torch.float32, device=self.device)
+        scores = torch.empty(B, self.nc, A, dtype=torch.float32, device=self.device)
+        sp = C.c_void_p(stream.cuda_stream) if stream is not None else C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        L.check(L.lib().yb_trainer_evaluate(self._h, C.c_void_p(images_nchw.data_ptr()),
+                                            L.YB_U8 if images_nchw.dtype == torch.uint8 else L.YB_F32, B,
+                                            *(C.c_void_p(t.data_ptr()) for t in (pred, boxes, scores)), sp))
+        return pred, boxes, scores
 
     def state_dict(self, dtype=torch.float32):
         """Reference-named tensors as `yolo.state_dict()` holds them (cf. TrainStepV8.state_dict)."""
