@@ -295,6 +295,41 @@ int32_t yb_get_grad(yb_trainer* t, const char* name, float* out_host, int64_t co
 int32_t yb_get_tensor(yb_trainer* t, const char* name, float* out_host, int64_t count);
 int32_t yb_trainer_evaluate(yb_trainer* t, const void* images, int32_t in_dtype, int32_t batch, float* pred, float* boxes,
                             float* scores, void* stream);
+/* The trainer's validation pass, `Detector.Val` (Models/Detector.cs:73-160) over a loader, on the device.
+ *   yb_trainer_val_begin   sizes trainer-owned accumulators (outside the activation arena) for at most max_images x 300
+ *                          detection rows and max_labels labels, and resets the rows, loss sums and image / label counts
+ *   yb_trainer_val_batch   one loader iteration (Detector.cs:81-132), images and targets as yb_train_backward: the eval
+ *                          forward of yb_trainer_evaluate, v8DetectionLoss without gradients added to the loss sums,
+ *                          non_max_suppression(conf 0.1, iou 0.7, max_det 300, max_nms 30000, max_wh 7680), the labels
+ *                          `xywh2xyxy(bboxes * (w, h, w, h))`, match_predictions at linspace(0.5, 0.95, 10) and the append of
+ *                          every image's kept rows (tp bits, conf, class) in image order.  Queued on `stream` without a host
+ *                          wait other than for the pinned target buffer (as yb_train_backward).  n_targets == 0: the batch is
+ *                          skipped (Detector.cs:91-94).  YB_ERR_INVALID_ARG for batch > max_batch, a class id outside
+ *                          [0, nc), more than 2048 labels in the batch, or more images / labels than val_begin was sized for;
+ *                          YB_ERR_STATE before val_begin.
+ *   yb_trainer_val_append  appends device rows in the accumulator layout: tp uint8 (n, 10), conf float32 (n), pred_cls
+ *                          int32 (n), target_cls int32 (m); the loss sums and the image count are not touched.  With
+ *                          yb_trainer_val_rows this merges the rows of data-parallel ranks before val_end.
+ *   yb_trainer_val_rows    HOST counts_host[2] = accumulated rows n and labels m (synchronises `stream`); when the device
+ *                          pointers are given (capacity n / m) the rows are copied there in the layout val_append takes;
+ *                          clear != 0 then empties the rows and labels (the loss sums and the image count stay)
+ *   yb_trainer_val_end     ap_per_class on the accumulated rows; synchronises.  HOST outputs: loss_items[3] the SUM of the
+ *                          executed batches' loss items (the reference's fitness is -sum of them); metrics[4] = P, R, mAP50,
+ *                          mAP50-95 with P = p.mean(), R = r.mean() over the classes that have labels, mAP50 = ap[:, 0].mean()
+ *                          and mAP50-95 = ap[:, 1:].mean() - the reference's Slice(1) leaves the 0.50 column out (Detector.cs:141);
+ *                          each mean summed in double and rounded to float32 once.  counts[3] = images, labels, detection rows.
+ *                          YB_ERR_STATE when no labels were accumulated (the reference's torch.cat of empty lists throws)
+ *                          or the rows overflowed.  Calling it again returns the same numbers.
+ * The pass changes no parameter, running statistic, gradient, Adam moment or BatchNorm ticket counter; like the step it is
+ * driven from one stream at a time. */
+int32_t yb_trainer_val_begin(yb_trainer* t, int32_t max_images, int32_t max_labels, void* stream);
+int32_t yb_trainer_val_batch(yb_trainer* t, const void* images, int32_t in_dtype, int32_t batch, const float* targets_host,
+                             int32_t n_targets, void* stream);
+int32_t yb_trainer_val_append(yb_trainer* t, const uint8_t* tp, const float* conf, const int32_t* pred_cls, int32_t n,
+                              const int32_t* target_cls, int32_t m, void* stream);
+int32_t yb_trainer_val_rows(yb_trainer* t, uint8_t* tp, float* conf, int32_t* pred_cls, int32_t* target_cls, int32_t* counts_host,
+                            int32_t clear, void* stream);
+int32_t yb_trainer_val_end(yb_trainer* t, float* loss_items_host, float* metrics_host, int32_t* counts_host, void* stream);
 
 /* Replaces (training path of YOLOv11, fp32 parity kernels): the forward and the autograd backward of the depthwise 3x3
  * convolutions - `Convs.DWConv` (Modules/Convs.cs:108-114; groups = gcd(c1, c2) = c for every use in Yolov11: the

@@ -87,6 +87,11 @@ SIGNATURES = {
     "yb_get_grad": (c_i32, [c_vp, c_cp, c_vp, C.c_int64]),
     "yb_get_tensor": (c_i32, [c_vp, c_cp, c_vp, C.c_int64]),
     "yb_trainer_evaluate": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "yb_trainer_val_begin": (c_i32, [c_vp, c_i32, c_i32, c_vp]),
+    "yb_trainer_val_batch": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp]),
+    "yb_trainer_val_append": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_vp]),
+    "yb_trainer_val_rows": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
+    "yb_trainer_val_end": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     "yb_stem_conv_forward_f32": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp]),
     "yb_stem_conv_backward_weight_f32": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, C.c_int64, c_vp]),
     "yb_dwconv3x3_forward_f32": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp]),

@@ -257,6 +257,23 @@ int detection_loss_prepare(const float* targets_host, int n_targets, int B, int 
 int detection_loss_launch_dev(const float* boxes, const float* scores, int B, int nc, int reg_max, int H, int W, const float* d_gts,
                               int n_max, int topk, float hyp_box, float hyp_cls, float hyp_dfl, float* loss_items, float* grad_boxes,
                               float* grad_scores, unsigned char* fg_out, int* gt_idx_out, float* tscore_out, cudaStream_t s);
+// val.cu : the per-batch tail of the trainer's validation pass (NMS -> labels -> matching -> append) and its accumulators
+// Detector.Val's max_det and IoU thresholds linspace(0.5, 0.95, 10); labels per batch: the matching kernel's shared arrays
+constexpr int VAL_MAX_DET = 300, VAL_T = 10, VAL_MAX_BATCH_LABELS = 2048;
+struct ValAccum {
+  unsigned char* tp;  // (cap_rows, VAL_T) correct bits
+  float* conf;        // (cap_rows)
+  int* cls;           // (cap_rows) predicted class
+  int* target_cls;    // (max_labels)
+  int* state;         // [0] rows appended so far, [1] overflow flag
+  float* loss;        // [3] summed loss items
+  long long cap_rows;
+};
+int val_batch_launch(const float* pred, int B, int nc, int A, int H, int W, const float* rows, int n_labels, long long label_off,
+                     const float* loss_detach, float* labels, float* dets, int* counts, unsigned char* correct, const ValAccum& acc,
+                     cudaStream_t s);
+int val_append_launch(const unsigned char* tp, const float* conf, const int* pred_cls, int n, const int* target_cls, int m,
+                      long long label_off, const ValAccum& acc, cudaStream_t s);
 // train_v11.cu : depthwise 3x3, stride 1, pad 1, fp32 NHWC
 int dwconv3x3_forward_f32(const float* x, const float* w, int N, int H, int W, int C, float* z, cudaStream_t s);
 int dwconv3x3_backward_f32(const float* x, const float* dz, const float* w, int N, int H, int W, int C, float* dx, float* dw,

@@ -796,6 +796,13 @@ struct yb_trainer {
   float* tg_pinned = nullptr;
   size_t tg_cap = 0;
   cudaEvent_t tg_copied = nullptr;
+  // validation pass (yb_trainer_val_*): the accumulators live outside the arena, which every call resets.  Images and labels
+  // are counted here; the detection row count and the loss sums only on the device (val.state / val.loss)
+  bool val_on = false;
+  ValAccum val{};
+  void* val_block = nullptr;
+  size_t val_bytes = 0;
+  int val_max_images = 0, val_max_labels = 0, val_images = 0, val_labels = 0;
 };
 
 namespace {
@@ -1015,6 +1022,28 @@ int forward_layers(yb_trainer* t, T4 x, T4 feats[3]) {
   return YB_OK;
 }
 
+// t->tg_host -> the pinned staging buffer -> the arena, queued on s.  The pinned buffer is reused by the next call: it is
+// only overwritten once the copy queued by the previous call has left it (tg_copied), the one host wait of a call.
+int stage_targets(yb_trainer* t, cudaStream_t s, const char* who, float** d_out) {
+  Net& n = t->net;
+  const std::string w(who);
+  if (!t->tg_copied && cudaEventCreateWithFlags(&t->tg_copied, cudaEventDisableTiming) != cudaSuccess) { set_error(w + ": cudaEventCreate failed"); return YB_ERR_CUDA; }
+  if (t->tg_pinned && cudaEventSynchronize(t->tg_copied) != cudaSuccess) { set_error(w + ": cudaEventSynchronize failed"); return YB_ERR_CUDA; }
+  if (t->tg_host.size() > t->tg_cap) {
+    if (t->tg_pinned) cudaFreeHost(t->tg_pinned);
+    t->tg_pinned = nullptr;
+    t->tg_cap = std::max<size_t>(t->tg_host.size() * 2, 4096);
+    if (cudaMallocHost((void**)&t->tg_pinned, t->tg_cap * sizeof(float)) != cudaSuccess) { t->tg_cap = 0; set_error(w + ": cudaMallocHost failed"); return YB_ERR_CUDA; }
+  }
+  memcpy(t->tg_pinned, t->tg_host.data(), t->tg_host.size() * sizeof(float));
+  float* d = n.alloc((long long)t->tg_host.size());
+  if (n.rc) return n.rc;
+  if (cudaMemcpyAsync(d, t->tg_pinned, t->tg_host.size() * sizeof(float), cudaMemcpyHostToDevice, s) != cudaSuccess ||
+      cudaEventRecord(t->tg_copied, s) != cudaSuccess) { set_error(w + ": target copy failed"); return YB_ERR_CUDA; }
+  *d_out = d;
+  return YB_OK;
+}
+
 // forward + loss + backward of one batch; gradients land in the caller's flat buffer
 int run_backward(yb_trainer* t, const void* images, int in_dtype, int B, const float* targets_host, int n_targets, float* items_host,
                  cudaStream_t s) {
@@ -1030,19 +1059,8 @@ int run_backward(yb_trainer* t, const void* images, int in_dtype, int B, const f
   // backward pass then started from an empty queue)
   int n_max = 0;
   if (int rc = detection_loss_prepare(targets_host, n_targets, B, n.nc, H, W, t->tg_host, &n_max)) return rc;
-  if (!t->tg_copied && cudaEventCreateWithFlags(&t->tg_copied, cudaEventDisableTiming) != cudaSuccess) { set_error("yb_train_step: cudaEventCreate failed"); return YB_ERR_CUDA; }
-  if (t->tg_pinned && cudaEventSynchronize(t->tg_copied) != cudaSuccess) { set_error("yb_train_step: cudaEventSynchronize failed"); return YB_ERR_CUDA; }
-  if (t->tg_host.size() > t->tg_cap) {
-    if (t->tg_pinned) cudaFreeHost(t->tg_pinned);
-    t->tg_pinned = nullptr;
-    t->tg_cap = std::max<size_t>(t->tg_host.size() * 2, 4096);
-    if (cudaMallocHost((void**)&t->tg_pinned, t->tg_cap * sizeof(float)) != cudaSuccess) { t->tg_cap = 0; set_error("yb_train_step: cudaMallocHost failed"); return YB_ERR_CUDA; }
-  }
-  memcpy(t->tg_pinned, t->tg_host.data(), t->tg_host.size() * sizeof(float));
-  float* d_gts = n.alloc((long long)t->tg_host.size());
-  if (n.rc) return n.rc;
-  if (cudaMemcpyAsync(d_gts, t->tg_pinned, t->tg_host.size() * sizeof(float), cudaMemcpyHostToDevice, s) != cudaSuccess ||
-      cudaEventRecord(t->tg_copied, s) != cudaSuccess) { set_error("yb_train_step: target copy failed"); return YB_ERR_CUDA; }
+  float* d_gts = nullptr;
+  if (int rc = stage_targets(t, s, "yb_train_step", &d_gts)) return rc;
   images_to_nhwc8_kernel<<<nb((long long)B * H * W), 256, 0, s>>>(images, in_dtype == YB_U8 ? 1 : 0, x.p, B, H, W);
   n.check_launch();
   n.check(tf_pack_all(n.P, n.WF, n.WB, n.pack_descs, n.n_packs, n.pack_chunks, s));  // the weights as this step sees them
@@ -1163,6 +1181,29 @@ int prepare_eval(yb_trainer* t) {
   return YB_OK;
 }
 
+int anchors(const Net& n) { return (n.H / 8) * (n.W / 8) + (n.H / 16) * (n.W / 16) + (n.H / 32) * (n.W / 32); }
+
+// the eval-mode forward (`AMPWrapper.Evaluate`) on the arena as the caller left it: one fold launch, then the layer walk
+// and the head with BatchNorm folded; pred / boxes / scores each optional
+int eval_forward(yb_trainer* t, const void* images, int in_dtype, int B, float* pred, float* boxes, float* scores) {
+  if (int rc = prepare_eval(t)) return rc;
+  Net& n = t->net;
+  T4 x = n.make(B, n.H, n.W, 8);
+  if (n.rc) return n.rc;
+  images_to_nhwc8_kernel<<<nb((long long)B * n.H * n.W), 256, 0, n.s>>>(images, in_dtype == YB_U8 ? 1 : 0, x.p, B, n.H, n.W);
+  n.check_launch();
+  n.check(tf_fold_all(n.fold_descs, n.n_folds, n.fold_chunks, n.s));  // BatchNorm as the current parameters and statistics give it
+  n.eval = true;
+  T4 feats[3];
+  int rc = forward_layers(t, x, feats);
+  if (!rc) {
+    t->detect->forward(n, feats, boxes, scores, anchors(n), pred);
+    rc = n.rc;
+  }
+  n.eval = false;
+  return rc;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1248,6 +1289,7 @@ void yb_trainer_destroy(yb_trainer* t) {
   if (t->net.fold_descs) cudaFree(t->net.fold_descs);
   if (t->tg_pinned) cudaFreeHost(t->tg_pinned);
   if (t->tg_copied) cudaEventDestroy(t->tg_copied);
+  if (t->val_block) cudaFree(t->val_block);
   delete t;
 }
 
@@ -1320,28 +1362,200 @@ int32_t yb_trainer_evaluate(yb_trainer* t, const void* images, int32_t in_dtype,
   if (batch <= 0 || batch > t->net.max_batch) { set_error("yb_trainer_evaluate: batch outside [1, max_batch]"); return YB_ERR_INVALID_ARG; }
   if (in_dtype != YB_U8 && in_dtype != YB_F32) { set_error("yb_trainer_evaluate: images must be u8 or f32 NCHW"); return YB_ERR_INVALID_ARG; }
   if (!have_device("yb_trainer_evaluate")) return YB_ERR_NO_DEVICE;
-  if (int rc = prepare_eval(t)) return rc;
   Net& n = t->net;
-  cudaStream_t s = (cudaStream_t)stream;
-  n.s = s;
+  n.s = (cudaStream_t)stream;
   n.rc = 0;
   n.arena_off = 0;
-  const int H = n.H, W = n.W;
-  T4 x = n.make(batch, H, W, 8);
-  if (n.rc) return n.rc;
-  images_to_nhwc8_kernel<<<nb((long long)batch * H * W), 256, 0, s>>>(images, in_dtype == YB_U8 ? 1 : 0, x.p, batch, H, W);
-  n.check_launch();
-  n.check(tf_fold_all(n.fold_descs, n.n_folds, n.fold_chunks, s));  // BatchNorm as the current parameters and statistics give it
-  n.eval = true;
-  T4 feats[3];
-  int rc = forward_layers(t, x, feats);
-  if (!rc) {
-    const int A = feats[0].H * feats[0].W + feats[1].H * feats[1].W + feats[2].H * feats[2].W;
-    t->detect->forward(n, feats, boxes, scores, A, pred);
-    rc = n.rc;
+  return eval_forward(t, images, in_dtype, batch, pred, boxes, scores);
+}
+
+int32_t yb_trainer_val_begin(yb_trainer* t, int32_t max_images, int32_t max_labels, void* stream) {
+  if (!t) { set_error("yb_trainer_val_begin: null trainer"); return YB_ERR_INVALID_ARG; }
+  if (!t->net.P || !t->net.arena) { set_error("yb_trainer_val_begin: call yb_trainer_bind first (and create without DRY_RUN)"); return YB_ERR_STATE; }
+  if (max_images <= 0 || max_labels <= 0 || (long long)max_images * VAL_MAX_DET > INT32_MAX) {
+    set_error("yb_trainer_val_begin: need max_images > 0 (at most 2^31 / 300) and max_labels > 0");
+    return YB_ERR_INVALID_ARG;
   }
-  n.eval = false;
-  return rc;
+  if (!have_device("yb_trainer_val_begin")) return YB_ERR_NO_DEVICE;
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t rows = (size_t)max_images * VAL_MAX_DET;
+  auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t o_conf = up(rows * VAL_T), o_cls = o_conf + up(rows * 4), o_tcls = o_cls + up(rows * 4),
+               o_state = o_tcls + up((size_t)max_labels * 4), bytes = o_state + 256;
+  t->val_on = false;
+  if (bytes > t->val_bytes) {
+    if (t->val_block) cudaFree(t->val_block);
+    t->val_block = nullptr;
+    t->val_bytes = 0;
+    if (cudaMalloc(&t->val_block, bytes) != cudaSuccess) {
+      t->val_block = nullptr;
+      cudaGetLastError();
+      set_error("yb_trainer_val_begin: cudaMalloc of the validation accumulators failed");
+      return YB_ERR_CUDA;
+    }
+    t->val_bytes = bytes;
+  }
+  char* b = static_cast<char*>(t->val_block);
+  ValAccum& a = t->val;
+  a.tp = reinterpret_cast<unsigned char*>(b);
+  a.conf = reinterpret_cast<float*>(b + o_conf);
+  a.cls = reinterpret_cast<int*>(b + o_cls);
+  a.target_cls = reinterpret_cast<int*>(b + o_tcls);
+  a.state = reinterpret_cast<int*>(b + o_state);
+  a.loss = reinterpret_cast<float*>(b + o_state + 16);
+  a.cap_rows = (long long)rows;
+  YB_CUDA_CHECK(cudaMemsetAsync(a.state, 0, 256, s));  // row count, overflow flag, loss sums
+  t->val_max_images = max_images;
+  t->val_max_labels = max_labels;
+  t->val_images = t->val_labels = 0;
+  t->val_on = true;
+  return YB_OK;
+}
+
+int32_t yb_trainer_val_batch(yb_trainer* t, const void* images, int32_t in_dtype, int32_t batch, const float* targets_host,
+                             int32_t n_targets, void* stream) {
+  if (!t || !images) { set_error("yb_trainer_val_batch: null argument"); return YB_ERR_INVALID_ARG; }
+  if (!t->val_on) { set_error("yb_trainer_val_batch: call yb_trainer_val_begin first"); return YB_ERR_STATE; }
+  if (batch <= 0 || batch > t->net.max_batch) { set_error("yb_trainer_val_batch: batch outside [1, max_batch]"); return YB_ERR_INVALID_ARG; }
+  if (in_dtype != YB_U8 && in_dtype != YB_F32) { set_error("yb_trainer_val_batch: images must be u8 or f32 NCHW"); return YB_ERR_INVALID_ARG; }
+  if (n_targets < 0 || (n_targets > 0 && !targets_host)) { set_error("yb_trainer_val_batch: bad targets"); return YB_ERR_INVALID_ARG; }
+  if (n_targets == 0) return YB_OK;  // Detector.cs:91-94: a batch without labels is skipped - no loss, rows or image count
+  if (t->val_images + batch > t->val_max_images || t->val_labels + n_targets > t->val_max_labels) {
+    set_error("yb_trainer_val_batch: more images or labels than yb_trainer_val_begin was sized for");
+    return YB_ERR_INVALID_ARG;
+  }
+  if (n_targets > VAL_MAX_BATCH_LABELS) { set_error("yb_trainer_val_batch: at most 2048 labels per batch"); return YB_ERR_INVALID_ARG; }
+  Net& n = t->net;
+  const int B = batch, H = n.H, W = n.W;
+  int n_max = 0;
+  // the loss's padded (B, n_max, 5) targets; validates image indices and class ids
+  if (int rc = detection_loss_prepare(targets_host, n_targets, B, n.nc, H, W, t->tg_host, &n_max)) return rc;
+  // followed by the raw rows, stably sorted by image: the order in which Detector.Val concatenates each image's labels
+  const size_t gts = t->tg_host.size();
+  std::vector<int> start(B + 1, 0);
+  for (int i = 0; i < n_targets; i++) start[(int)targets_host[(size_t)i * 6] + 1]++;
+  for (int b = 0; b < B; b++) start[b + 1] += start[b];
+  t->tg_host.resize(gts + (size_t)n_targets * 6);
+  for (int i = 0; i < n_targets; i++) {
+    const float* r = targets_host + (size_t)i * 6;
+    std::copy(r, r + 6, t->tg_host.begin() + gts + (size_t)start[(int)r[0]]++ * 6);
+  }
+  n.s = (cudaStream_t)stream;
+  n.rc = 0;
+  n.arena_off = 0;
+  float* d_tg = nullptr;
+  if (int rc = stage_targets(t, n.s, "yb_trainer_val_batch", &d_tg)) return rc;
+  const int A = anchors(n);
+  float* pred = n.alloc((long long)B * (4 + n.nc) * A);
+  float* boxes = n.alloc((long long)B * 64 * A);
+  float* scores = n.alloc((long long)B * n.nc * A);
+  float* items = n.alloc(4);
+  float* labels = n.alloc((long long)n_targets * 6);
+  float* dets = n.alloc((long long)B * VAL_MAX_DET * 6);
+  int* counts = reinterpret_cast<int*>(n.alloc(B));
+  unsigned char* correct = reinterpret_cast<unsigned char*>(n.alloc(((long long)B * VAL_MAX_DET * VAL_T + 3) / 4));
+  if (n.rc) return n.rc;
+  if (int rc = eval_forward(t, images, in_dtype, B, pred, boxes, scores)) return rc;
+  // v8DetectionLoss without gradients: `loss.forward(preds, data).loss_detach` (Detector.cs:96)
+  if (int rc = detection_loss_launch_dev(boxes, scores, B, n.nc, 16, H, W, d_tg, n_max, 10, 7.5f, 0.5f, 1.5f, items, nullptr, nullptr,
+                                         nullptr, nullptr, nullptr, n.s))
+    return rc;
+  if (int rc = val_batch_launch(pred, B, n.nc, A, H, W, d_tg + gts, n_targets, t->val_labels, items, labels, dets, counts, correct, t->val,
+                                n.s))
+    return rc;
+  t->val_images += B;
+  t->val_labels += n_targets;
+  return YB_OK;
+}
+
+int32_t yb_trainer_val_append(yb_trainer* t, const uint8_t* tp, const float* conf, const int32_t* pred_cls, int32_t n,
+                              const int32_t* target_cls, int32_t m, void* stream) {
+  if (!t) { set_error("yb_trainer_val_append: null trainer"); return YB_ERR_INVALID_ARG; }
+  if (!t->val_on) { set_error("yb_trainer_val_append: call yb_trainer_val_begin first"); return YB_ERR_STATE; }
+  if (n < 0 || m < 0 || (n > 0 && (!tp || !conf || !pred_cls)) || (m > 0 && !target_cls)) { set_error("yb_trainer_val_append: bad argument"); return YB_ERR_INVALID_ARG; }
+  if (t->val_labels + m > t->val_max_labels) { set_error("yb_trainer_val_append: more labels than yb_trainer_val_begin was sized for"); return YB_ERR_INVALID_ARG; }
+  if (n == 0 && m == 0) return YB_OK;
+  if (int rc = val_append_launch(tp, conf, pred_cls, n, target_cls, m, t->val_labels, t->val, (cudaStream_t)stream)) return rc;
+  t->val_labels += m;
+  return YB_OK;
+}
+
+int32_t yb_trainer_val_rows(yb_trainer* t, uint8_t* tp, float* conf, int32_t* pred_cls, int32_t* target_cls, int32_t* counts_host,
+                            int32_t clear, void* stream) {
+  if (!t || !counts_host) { set_error("yb_trainer_val_rows: null argument"); return YB_ERR_INVALID_ARG; }
+  if (!t->val_on) { set_error("yb_trainer_val_rows: call yb_trainer_val_begin first"); return YB_ERR_STATE; }
+  cudaStream_t s = (cudaStream_t)stream;
+  int st[2] = {0, 0};
+  YB_CUDA_CHECK(cudaMemcpyAsync(st, t->val.state, sizeof(st), cudaMemcpyDeviceToHost, s));
+  YB_CUDA_CHECK(cudaStreamSynchronize(s));
+  if (st[1]) { set_error("yb_trainer_val_rows: the detection rows overflowed the accumulators"); return YB_ERR_STATE; }
+  const int n = st[0], m = t->val_labels;
+  counts_host[0] = n;
+  counts_host[1] = m;
+  if (tp && n) YB_CUDA_CHECK(cudaMemcpyAsync(tp, t->val.tp, (size_t)n * VAL_T, cudaMemcpyDeviceToDevice, s));
+  if (conf && n) YB_CUDA_CHECK(cudaMemcpyAsync(conf, t->val.conf, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
+  if (pred_cls && n) YB_CUDA_CHECK(cudaMemcpyAsync(pred_cls, t->val.cls, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
+  if (target_cls && m) YB_CUDA_CHECK(cudaMemcpyAsync(target_cls, t->val.target_cls, (size_t)m * 4, cudaMemcpyDeviceToDevice, s));
+  if (clear) {
+    YB_CUDA_CHECK(cudaMemsetAsync(t->val.state, 0, sizeof(int), s));  // the row count; loss sums and the image count stay
+    t->val_labels = 0;
+  }
+  return YB_OK;
+}
+
+int32_t yb_trainer_val_end(yb_trainer* t, float* loss_items_host, float* metrics_host, int32_t* counts_host, void* stream) {
+  if (!t || !loss_items_host || !metrics_host || !counts_host) { set_error("yb_trainer_val_end: null argument"); return YB_ERR_INVALID_ARG; }
+  if (!t->val_on) { set_error("yb_trainer_val_end: call yb_trainer_val_begin first"); return YB_ERR_STATE; }
+  // every executed batch has labels, so no labels means nothing was accumulated (the reference's torch.cat of empty lists throws)
+  if (t->val_labels == 0) { set_error("yb_trainer_val_end: no batch with labels was validated"); return YB_ERR_STATE; }
+  cudaStream_t s = (cudaStream_t)stream;
+  struct { int st[4]; float loss[3]; } h{};
+  static_assert(sizeof(h) == 28, "state block layout");
+  YB_CUDA_CHECK(cudaMemcpyAsync(&h, t->val.state, sizeof(h), cudaMemcpyDeviceToHost, s));
+  YB_CUDA_CHECK(cudaStreamSynchronize(s));
+  if (h.st[1]) { set_error("yb_trainer_val_end: the detection rows overflowed the accumulators"); return YB_ERR_STATE; }
+  const int n = h.st[0], m = t->val_labels, nc = t->net.nc, T = VAL_T;
+  // ap_per_class outputs: unique | ap | p_curve | r_curve | f1_curve | prec_values | p | r | f1 | tp | fp
+  float* o = nullptr;
+  const size_t fl = (size_t)nc * (1 + T + 4 * 1000 + 5);
+  YB_CUDA_CHECK(cudaMallocAsync((void**)&o, fl * 4, s));
+  int* uniq = reinterpret_cast<int*>(o);
+  float* ap = o + nc;
+  float* curves = ap + (size_t)nc * T;
+  float* p = curves + (size_t)nc * 4000;
+  float* r = p + nc;
+  int counts[3] = {0, 0, 0};
+  int rc = yb_ap_per_class(t->val.tp, t->val.conf, t->val.cls, n, T, t->val.target_cls, m, nc, uniq, counts, ap, curves, curves + nc * 1000,
+                           curves + nc * 2000, curves + nc * 3000, p, r, r + nc, r + 2 * nc, r + 3 * nc, s);
+  std::vector<float> hp(nc), hr(nc), hap((size_t)nc * T);
+  const int nu = counts[0];  // classes with labels: rows [0, nu) of the outputs
+  if (!rc && (cudaMemcpyAsync(hp.data(), p, (size_t)nu * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+              cudaMemcpyAsync(hr.data(), r, (size_t)nu * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+              cudaMemcpyAsync(hap.data(), ap, (size_t)nu * T * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+              cudaStreamSynchronize(s) != cudaSuccess)) {
+    set_error(std::string("yb_trainer_val_end: ") + cudaGetErrorString(cudaGetLastError()));
+    rc = YB_ERR_CUDA;
+  }
+  cudaFreeAsync(o, s);
+  if (rc) return rc;
+  // P = p.mean(), R = r.mean(), mAP50 = ap[:, 0].mean(), mAP50-95 = ap[:, 1:].mean() (Detector.cs:138-141: the reference's
+  // Slice(1) leaves the 0.50 column out of mAP50-95); each mean summed in double and rounded to fp32 once
+  double sp = 0, sr = 0, s50 = 0, s95 = 0;
+  for (int c = 0; c < nu; c++) {
+    sp += hp[c];
+    sr += hr[c];
+    s50 += hap[(size_t)c * T];
+    for (int j = 1; j < T; j++) s95 += hap[(size_t)c * T + j];
+  }
+  metrics_host[0] = (float)(sp / nu);
+  metrics_host[1] = (float)(sr / nu);
+  metrics_host[2] = (float)(s50 / nu);
+  metrics_host[3] = (float)(s95 / ((double)nu * (T - 1)));
+  for (int i = 0; i < 3; i++) loss_items_host[i] = h.loss[i];
+  counts_host[0] = t->val_images;
+  counts_host[1] = m;
+  counts_host[2] = n;
+  return YB_OK;
 }
 
 int32_t yb_get_grad(yb_trainer* t, const char* name, float* out_host, int64_t count) {

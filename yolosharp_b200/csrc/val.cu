@@ -101,6 +101,122 @@ __global__ void __launch_bounds__(256) mask_iou_kernel(const float* __restrict__
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The per-batch tail of the trainer's validation pass (yb_trainer_val_batch, Models/Detector.cs:81-132) and its
+// accumulators.  The running row count lives on the device, so a batch is queued without the host learning how many
+// detections NMS kept; the host counts images and labels itself and passes the label offset in.
+// ---------------------------------------------------------------------------------------------------------------
+
+// staged target rows [image, cls, x, y, w, h] (normalised, sorted by image) -> labels [image, cls, x1, y1, x2, y2] in input
+// pixels, in the reference's order: `bboxes * (w, h, w, h)` then `Ops.xywh2xyxy` (Ops.cs:68-81) - the same fp32 operations
+// as oracle/ops.py; and the int32 class of every label into the accumulator
+__global__ void val_labels_kernel(const float* __restrict__ rows, int n, float W, float H, float* __restrict__ labels,
+                                  int* __restrict__ target_cls) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float* r = rows + (size_t)i * 6;
+  const float x = __fmul_rn(r[2], W), y = __fmul_rn(r[3], H), w = __fmul_rn(r[4], W), h = __fmul_rn(r[5], H);
+  float* o = labels + (size_t)i * 6;
+  o[0] = r[0];
+  o[1] = r[1];
+  o[2] = __fsub_rn(x, __fdiv_rn(w, 2.f));
+  o[3] = __fsub_rn(y, __fdiv_rn(h, 2.f));
+  o[4] = __fadd_rn(x, __fdiv_rn(w, 2.f));
+  o[5] = __fadd_rn(y, __fdiv_rn(h, 2.f));
+  target_cls[i] = (int)r[1];
+}
+
+// one CTA: the kept NMS rows of every image, in image order and score order within an image, appended at the device row
+// counter; and `loss_items = loss_items + loss_detach` (Detector.cs:124).  A batch that would not fit raises the overflow
+// flag and appends nothing.
+__global__ void __launch_bounds__(1024) val_accumulate_kernel(const float* __restrict__ dets, const int* __restrict__ counts, int B,
+                                                              const unsigned char* __restrict__ correct,
+                                                              const float* __restrict__ loss_detach, ValAccum acc) {
+  extern __shared__ int off[];  // B + 1 row offsets
+  const int base = acc.state[0];
+  if (threadIdx.x == 0) {
+    int o = 0;
+    for (int b = 0; b < B; b++) { off[b] = o; o += min(counts[b], VAL_MAX_DET); }
+    off[B] = o;
+  }
+  if (threadIdx.x < 3) acc.loss[threadIdx.x] = __fadd_rn(acc.loss[threadIdx.x], loss_detach[threadIdx.x]);
+  __syncthreads();
+  const int total = off[B];
+  if ((long long)base + total > acc.cap_rows) {
+    if (threadIdx.x == 0) acc.state[1] = 1;
+    return;
+  }
+  for (int i = threadIdx.x; i < total; i += blockDim.x) {
+    int lo = 0, hi = B - 1;  // the image of output row i: the last b with off[b] <= i
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (off[mid] <= i) lo = mid; else hi = mid - 1;
+    }
+    const size_t src = (size_t)lo * VAL_MAX_DET + (i - off[lo]);
+    const size_t dst = (size_t)base + i;
+#pragma unroll
+    for (int t = 0; t < VAL_T; t++) acc.tp[dst * VAL_T + t] = correct[src * VAL_T + t];
+    acc.conf[dst] = dets[src * 6 + 4];
+    acc.cls[dst] = (int)dets[src * 6 + 5];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) acc.state[0] = base + total;
+}
+
+// one CTA: rows already in the accumulator layout (another rank's, gathered by the host) appended at the row counter, and
+// their labels' classes at the host-known label offset
+__global__ void __launch_bounds__(1024) val_append_rows_kernel(const unsigned char* __restrict__ tp, const float* __restrict__ conf,
+                                                               const int* __restrict__ pred_cls, int n, const int* __restrict__ target_cls,
+                                                               int m, long long label_off, ValAccum acc) {
+  const int base = acc.state[0];
+  for (int i = threadIdx.x; i < m; i += blockDim.x) acc.target_cls[label_off + i] = target_cls[i];
+  if ((long long)base + n > acc.cap_rows) {
+    if (threadIdx.x == 0) acc.state[1] = 1;
+    return;
+  }
+  for (long long i = threadIdx.x; i < (long long)n * VAL_T; i += blockDim.x) acc.tp[(size_t)base * VAL_T + i] = tp[i];
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    acc.conf[(size_t)base + i] = conf[i];
+    acc.cls[(size_t)base + i] = pred_cls[i];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) acc.state[0] = base + n;
+}
+
+// Detector.Val's IoU vector torch.linspace(0.5, 0.95, 10) as ATen computes it in float32: the step rounded once, each value
+// one rounding of start + step * i (first half) or end - step * (steps - 1 - i) (second half)
+static MatchThr val_iouv() {
+  MatchThr t;
+  const float step = (0.95f - 0.5f) / 9.f;
+  for (int i = 0; i < MP_MAX_THR; i++)
+    t.v[i] = i >= VAL_T ? 2.f : (float)(i < 5 ? 0.5 + (double)step * i : (double)0.95f - (double)step * (VAL_T - 1 - i));
+  return t;
+}
+
+int val_batch_launch(const float* pred, int B, int nc, int A, int H, int W, const float* rows, int n_labels, long long label_off,
+                     const float* loss_detach, float* labels, float* dets, int* counts, unsigned char* correct, const ValAccum& acc,
+                     cudaStream_t s) {
+  static_assert(VAL_MAX_BATCH_LABELS == MP_MAX_LABELS, "the matching kernel's label limit");
+  // these kernels follow ordinary launches (the loss, NMS and matching kernels), so they are launched the ordinary way
+  val_labels_kernel<<<(n_labels + 255) / 256, 256, 0, s>>>(rows, n_labels, (float)W, (float)H, labels, acc.target_cls + label_off);
+  YB_CUDA_CHECK(cudaGetLastError());
+  // Ops.non_max_suppression(inference["boxes"], nc, conf_thres: 0.1, iou_thres: 0.7) with the defaults max_det 300,
+  // max_nms 30000, max_wh 7680 (Detector.cs:97)
+  if (int rc = nms_launch(pred, B, 4 + nc, A, nc, 0.1f, 0.7f, VAL_MAX_DET, 30000, 7680, dets, counts, nullptr, s)) return rc;
+  match_predictions_kernel<<<dim3(B, VAL_T), 256, 0, s>>>(dets, counts, VAL_MAX_DET, 6, labels, n_labels, val_iouv(), VAL_T, correct);
+  YB_CUDA_CHECK(cudaGetLastError());
+  val_accumulate_kernel<<<1, 1024, (B + 1) * sizeof(int), s>>>(dets, counts, B, correct, loss_detach, acc);
+  YB_CUDA_CHECK(cudaGetLastError());
+  return YB_OK;
+}
+
+int val_append_launch(const unsigned char* tp, const float* conf, const int* pred_cls, int n, const int* target_cls, int m,
+                      long long label_off, const ValAccum& acc, cudaStream_t s) {
+  val_append_rows_kernel<<<1, 1024, 0, s>>>(tp, conf, pred_cls, n, target_cls, m, label_off, acc);
+  YB_CUDA_CHECK(cudaGetLastError());
+  return YB_OK;
+}
+
 }  // namespace yb
 
 using namespace yb;

@@ -114,15 +114,8 @@ class NativeTrainer:
         B <= max_batch at the trainer's H x W.  Changes no parameter, running statistic, gradient or Adam moment.
         -> (pred (B, 4+nc, A) decoded xywh + class probabilities, boxes (B, 64, A), scores (B, nc, A) raw head outputs),
         device tensors written on `stream` (default: the current stream)."""
-        if not (torch.is_tensor(images_nchw) and images_nchw.dim() == 4 and images_nchw.shape[1] == 3 and
-                images_nchw.dtype in (torch.uint8, torch.float32)):
-            raise ValueError("evaluate: images must be a (B, 3, H, W) uint8 or float32 tensor")
+        self._check_images(images_nchw, "evaluate")
         B, _, H, W = images_nchw.shape
-        if B < 1 or B > self.max_batch or (H, W) != (self.height, self.width):
-            raise ValueError(f"evaluate: batch {B} x {H} x {W}, the trainer takes 1..{self.max_batch} x {self.height} x {self.width}")
-        if self.device.type != "cuda":
-            raise RuntimeError("evaluate: this trainer was created without a device (layout only)")
-        assert images_nchw.is_cuda and images_nchw.is_contiguous()
         A = sum((H // s) * (W // s) for s in (8, 16, 32))
         pred = torch.empty(B, 4 + self.nc, A, dtype=torch.float32, device=self.device)
         boxes = torch.empty(B, 64, A, dtype=torch.float32, device=self.device)
@@ -132,6 +125,84 @@ class NativeTrainer:
                                             L.YB_U8 if images_nchw.dtype == torch.uint8 else L.YB_F32, B,
                                             *(C.c_void_p(t.data_ptr()) for t in (pred, boxes, scores)), sp))
         return pred, boxes, scores
+
+    def _check_images(self, images_nchw, who):
+        if not (torch.is_tensor(images_nchw) and images_nchw.dim() == 4 and images_nchw.shape[1] == 3 and
+                images_nchw.dtype in (torch.uint8, torch.float32)):
+            raise ValueError(f"{who}: images must be a (B, 3, H, W) uint8 or float32 tensor")
+        B, _, H, W = images_nchw.shape
+        if B < 1 or B > self.max_batch or (H, W) != (self.height, self.width):
+            raise ValueError(f"{who}: batch {B} x {H} x {W}, the trainer takes 1..{self.max_batch} x {self.height} x {self.width}")
+        if self.device.type != "cuda":
+            raise RuntimeError(f"{who}: this trainer was created without a device (layout only)")
+        assert images_nchw.is_cuda and images_nchw.is_contiguous()
+
+    def validate(self, batches, group=None):
+        """`Detector.Val` (Models/Detector.cs:73-160) over `batches`, a re-iterable of (images, targets) as `step` takes them,
+        on the current stream: yb_trainer_val_begin, yb_trainer_val_batch per batch (a batch without targets is skipped),
+        yb_trainer_val_end.  -> (loss_items (3,), metrics (4,)) host float32: the SUM of the executed batches' loss items
+        and P, R, mAP50, mAP50-95 (mAP50-95 = ap[:, 1:].mean(), the reference's Slice(1)).  `last_val_counts` keeps
+        (images, labels, detection rows).
+        Data-parallel (an initialised torch.distributed `group` - default: this trainer's - of world > 1): every rank
+        validates its own shard, then gathers all ranks' detection rows and labels and rebuilds its accumulators in rank
+        order (rank 0's rows, then rank 1's, ...), so that every rank runs ap_per_class on the same rows in the same order
+        (it breaks confidence ties by input order) and reports the same metrics as one device validating the rank-order
+        concatenation of the shards.  The loss items and the image count stay per rank: `train.fit` all-reduces the
+        fitness itself."""
+        group = self.group if group is None else group
+        lib, dev = L.lib(), self.device
+        batches = [(x, torch.as_tensor(t, dtype=torch.float32).reshape(-1, 6).cpu().contiguous()) for x, t in batches]
+        for x, _ in batches:
+            self._check_images(x, "validate")
+        dp = group is not False and torch.distributed.is_available() and torch.distributed.is_initialized() and \
+            torch.distributed.get_world_size(group) > 1
+        size = torch.tensor([sum(int(x.shape[0]) for x, t in batches if len(t)), sum(len(t) for _, t in batches)], dtype=torch.int64)
+        if dp:  # the merged accumulators hold every rank's rows
+            size = size.to(dev)
+            torch.distributed.all_reduce(size, group=group)
+            size = size.cpu()
+        sp = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        L.check(lib.yb_trainer_val_begin(self._h, max(int(size[0]), 1), max(int(size[1]), 1), sp))
+        for x, t in batches:
+            L.check(lib.yb_trainer_val_batch(self._h, C.c_void_p(x.data_ptr()), L.YB_U8 if x.dtype == torch.uint8 else L.YB_F32,
+                                              x.shape[0], C.c_void_p(t.data_ptr()) if len(t) else None, len(t), sp))
+        if dp:
+            self._merge_val_rows(group, sp)
+        items, metrics, counts = torch.empty(3), torch.empty(4), torch.zeros(3, dtype=torch.int32)
+        L.check(lib.yb_trainer_val_end(self._h, *(C.c_void_p(v.data_ptr()) for v in (items, metrics, counts)), sp))
+        self.last_val_counts = tuple(int(v) for v in counts)
+        return items, metrics
+
+    def _merge_val_rows(self, group, sp):
+        """Replace this rank's accumulated rows by all ranks' rows in rank order (the loss sums and image count stay)."""
+        lib, dev, dist = L.lib(), self.device, torch.distributed
+        nm = torch.zeros(2, dtype=torch.int32)
+        L.check(lib.yb_trainer_val_rows(self._h, None, None, None, None, C.c_void_p(nm.data_ptr()), 0, sp))
+        world = dist.get_world_size(group)
+        sizes = [torch.zeros(2, dtype=torch.int32, device=dev) for _ in range(world)]
+        dist.all_gather(sizes, nm.to(dev), group=group)
+        sizes = [tuple(int(v) for v in s.cpu()) for s in sizes]
+        N, M = max(max(s[0] for s in sizes), 1), max(max(s[1] for s in sizes), 1)
+        mine = (torch.zeros((N, 10), dtype=torch.uint8, device=dev), torch.zeros(N, device=dev),
+                torch.zeros(N, dtype=torch.int32, device=dev), torch.zeros(M, dtype=torch.int32, device=dev))
+        L.check(lib.yb_trainer_val_rows(self._h, *(C.c_void_p(v.data_ptr()) for v in mine), C.c_void_p(nm.data_ptr()), 1, sp))
+        gathered = []
+        for t in mine:
+            parts = [torch.empty_like(t) for _ in range(world)]
+            dist.all_gather(parts, t, group=group)
+            gathered.append(parts)
+        for r, (n, m) in enumerate(sizes):
+            tp, conf, cls, tcls = (g[r] for g in gathered)
+            L.check(lib.yb_trainer_val_append(self._h, C.c_void_p(tp.data_ptr()), C.c_void_p(conf.data_ptr()), C.c_void_p(cls.data_ptr()),
+                                              n, C.c_void_p(tcls.data_ptr()), m, sp))
+
+    def validator(self, batches, group=None):
+        """The `validate(epoch)` callback of `train.fit`: runs `validate(batches, group)` and returns its loss items
+        (fit's fitness is -sum of them, YoloBaseTaskModel.cs:186); the metrics of the last pass are kept in `val_metrics`."""
+        def run(epoch):
+            items, self.val_metrics = self.validate(batches, group)
+            return items
+        return run
 
     def state_dict(self, dtype=torch.float32):
         """Reference-named tensors as `yolo.state_dict()` holds them (cf. TrainStepV8.state_dict)."""
